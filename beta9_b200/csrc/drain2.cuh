@@ -893,8 +893,10 @@ __device__ __noinline__ void group_copy_staged(uint8_t* dst, const uint8_t* src,
 template <int G>
 __device__ __noinline__ void group_copy_generic(uint8_t* dst, const uint8_t* src, uint32_t n, int sub) { group_copy<G>(dst, src, n, sub); }
 
+// (identity's main loop never holds a float64 / container record: those tasks are deferred to slow_task, which calls
+// seq_emit<true> itself; leaving the call out of the loop keeps configs[1]'s kernel as it was)
 template <int HANDLER>
-__device__ __forceinline__ void d2_phase_b_task(const uint8_t* __restrict__ p, const TaskRec& rec, uint8_t* __restrict__ o) { seq_emit(p, rec, o); }
+__device__ __forceinline__ void d2_phase_b_task(const uint8_t* __restrict__ p, const TaskRec& rec, uint8_t* __restrict__ o) { seq_emit<HANDLER == 3>(p, rec, o); }
 
 // the sequential validating parser + handler sizing, out of line: rare for identity, and it keeps the
 // hot loops' registers and instruction-cache footprint small
@@ -1271,7 +1273,7 @@ __device__ __noinline__ void slow_task(const DrainArgs& a, uint64_t goff, uint32
             else      esc_emit_general(p + FRAME_PRE_LEN, nbody, lane, o, L);
         }
         else if (rec.mode == OM_COPY) warp_copy(o, p + rec.src_off, rec.src_len, lane);
-        else if (lane == 0) d2_phase_b_task<0>(p, rec, o);
+        else if (lane == 0) seq_emit<true>(p, rec, o);
     }
     if (lane == 0) { a.out_off[j] = fits ? base : 0; a.out_len[j] = rec.out_len; a.out_status[j] = rec.status; a.out_has[j] = rec.has; }
     __syncwarp();

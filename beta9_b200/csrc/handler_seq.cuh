@@ -13,44 +13,17 @@ namespace b9 {
 // what phase A leaves for phase B, per task of the tile
 enum OutMode : uint8_t { OM_NONE = 0, OM_COPY, OM_STR_ESC /* one thread walks the token */, OM_U32_DEC, OM_I64_DEC, OM_VADD,
                          OM_STR_PAR /* warp transcodes the framed body in 32 chunks (drain2) */,
-                         OM_DEFER /* identity main kernel: left to drain_slow_kernel */ };
+                         OM_DEFER /* identity main kernel: left to drain_slow_kernel */,
+                         OM_PY_NUM /* identity of a number: py_json_go_number(value) */,
+                         OM_PY_FLOAT /* json_sum's float result: py_json_float(value) */,
+                         OM_PY_VALUE /* identity of a non-empty list / object: py_value_json over the token */ };
 struct TaskRec {
-    uint32_t src_off;    // OM_COPY / OM_STR_ESC / OM_VADD: byte offset inside the payload
+    uint32_t src_off;    // OM_COPY / OM_STR_ESC / OM_VADD / OM_PY_VALUE: byte offset inside the payload
     uint32_t src_len;
     uint32_t out_len;
     uint8_t  status, has, mode, ready;
-    long long value;     // OM_U32_DEC / OM_I64_DEC
+    long long value;     // OM_U32_DEC / OM_I64_DEC; the float64's bits for OM_PY_NUM / OM_PY_FLOAT
 };
-
-// decimal digits of v. (Round 1 divided by ten in 64 bits, one lane per task while 31 idle: 6-9 % of the crc32 and json_sum
-// kernels' instructions went into printing ~10 digits. Now: compares against powers
-// of ten and 32-bit multiply-shift division by 10, in at most three 9-digit limbs.)
-__device__ __forceinline__ uint32_t dec_len_u32(uint32_t v) {
-    return 1u + (v >= 10u) + (v >= 100u) + (v >= 1000u) + (v >= 10000u) + (v >= 100000u) + (v >= 1000000u) + (v >= 10000000u) + (v >= 100000000u) + (v >= 1000000000u);
-}
-__device__ __forceinline__ uint32_t dec_len_u64(unsigned long long v) {
-    if (v < 4294967296ull) return dec_len_u32((uint32_t)v);
-    const unsigned long long hi = v / 1000000000ull;                    // >= 4: v has more than 9 digits
-    if (hi < 4294967296ull) return 9u + dec_len_u32((uint32_t)hi);
-    return 18u + dec_len_u32((uint32_t)(hi / 1000000000ull));
-}
-// exactly n digits of x (x < 10^n), most significant first, zero-padded on the left
-__device__ __forceinline__ void write_dec_u32(uint8_t* o, uint32_t x, uint32_t n) {
-    for (uint32_t k = n; k-- > 0;) {
-        const uint32_t q = (uint32_t)(((unsigned long long)x * 0xCCCCCCCDull) >> 35);   // x / 10
-        o[k] = (uint8_t)('0' + (x - q * 10u));
-        x = q;
-    }
-}
-__device__ inline void write_dec(uint8_t* o, unsigned long long v, uint32_t len) {
-    if (v < 4294967296ull) { write_dec_u32(o, (uint32_t)v, len); return; }
-    const unsigned long long hi = v / 1000000000ull;
-    write_dec_u32(o + (len - 9u), (uint32_t)(v - hi * 1000000000ull), 9u);
-    if (hi < 4294967296ull) { write_dec_u32(o, (uint32_t)hi, len - 9u); return; }
-    const unsigned long long top = hi / 1000000000ull;
-    write_dec_u32(o + (len - 18u), (uint32_t)(hi - top * 1000000000ull), 9u);
-    write_dec_u32(o, (uint32_t)top, len - 18u);
-}
 
 // String token p[s..e) (quotes included, validated): does the Python-escaped form equal a plain
 // copy?  Computes the json.dumps length either way. One thread.
@@ -58,6 +31,98 @@ __device__ inline uint32_t py_string_len(const uint8_t* __restrict__ p, uint32_t
     uint32_t i = s + 1, end = e - 1, out = 2;
     while (i < end) out += py_escaped_len(next_cp(p, i, end));
     return out;
+}
+__device__ inline uint32_t py_string_write(const uint8_t* __restrict__ p, uint32_t s, uint32_t e, uint8_t* __restrict__ o) {
+    uint32_t i = s + 1, end = e - 1, n = 1;
+    o[0] = '"';
+    while (i < end) n += py_emit(next_cp(p, i, end), o + n);
+    o[n] = '"';
+    return n + 1;
+}
+
+// json.dumps of the value Go decodes from the validated, non-empty JSON list or object p[s..e), as the runner's
+// json.loads reads it back from Go's encoding: separators ", " and ": ", strings by py_emit (ensure_ascii), numbers
+// by py_json_go_number, object members in Go's map order -- keys sorted bytewise by their decoded UTF-8, the last
+// of duplicate keys winning. That order needs no storage: each step scans the object for the smallest key after the
+// one emitted last (among equal keys the last occurrence), which is quadratic in the member count.
+// o == nullptr: size only. Returns the byte count, or -1 where the device DECLINES: nesting deeper than
+// PY_VALUE_MAX_DEPTH, an object with more than PY_VALUE_MAX_MEMBERS members, a number f64_parse cannot settle.
+constexpr int PY_VALUE_MAX_DEPTH = 16;
+constexpr uint32_t PY_VALUE_MAX_MEMBERS = 64;
+__device__ __noinline__ int64_t py_value_json(const uint8_t* __restrict__ p, uint32_t s, uint32_t e, uint8_t* __restrict__ o) {
+    uint32_t pos[PY_VALUE_MAX_DEPTH];              // list: the next element (or ','); object: just past its '{'
+    uint32_t lks[PY_VALUE_MAX_DEPTH], lke[PY_VALUE_MAX_DEPTH];   // object: body of the key emitted last
+    uint32_t is_obj = 0, started = 0;              // bit d: the container at depth d is an object / has emitted a member
+    int depth = 0;
+    int64_t n = 0;
+    uint32_t vs = s, ve = e;                       // the value to emit next
+    bool have = true;
+    for (;;) {
+        if (have) {
+            have = false;
+            const uint8_t c = p[vs];
+            if (c == '{' || c == '[') {
+                if (o) o[n] = c;
+                ++n;
+                if (only_ws(p, vs + 1, ve - 1)) { if (o) o[n] = (c == '{') ? '}' : ']'; ++n; }
+                else {
+                    if (depth == PY_VALUE_MAX_DEPTH) return -1;
+                    const uint32_t bit = 1u << depth;
+                    pos[depth] = vs + 1; started &= ~bit;
+                    if (c == '{') is_obj |= bit; else is_obj &= ~bit;
+                    ++depth;
+                }
+            } else if (c == '"') n += o ? py_string_write(p, vs, ve, o + n) : py_string_len(p, vs, ve);
+            else if (c == 't' || c == 'n') { if (o) for (int k = 0; k < 4; ++k) o[n + k] = p[vs + k]; n += 4; }
+            else if (c == 'f') { if (o) for (int k = 0; k < 5; ++k) o[n + k] = p[vs + k]; n += 5; }
+            else {
+                unsigned long long b = 0;
+                if (!f64_parse(p, vs, ve, &b)) return -1;
+                n += py_json_go_number(b, o ? o + n : nullptr);
+            }
+        }
+        if (depth == 0) return n;
+        const int d = depth - 1;
+        const uint32_t bit = 1u << d;
+        uint32_t f = 0;
+        if (!(is_obj & bit)) {                     // list: the next element in order
+            uint32_t i = pos[d];
+            while (is_ws(p[i])) ++i;
+            if (p[i] == ']') { if (o) o[n] = ']'; ++n; --depth; continue; }
+            if (p[i] == ',') { ++i; while (is_ws(p[i])) ++i; }
+            if (started & bit) { if (o) { o[n] = ','; o[n + 1] = ' '; } n += 2; }
+            started |= bit;
+            vs = i; ve = (uint32_t)skip_value(p, i, e, f); pos[d] = ve; have = true;
+            continue;
+        }
+        // object: the smallest key after the last one emitted
+        uint32_t i = pos[d], members = 0, bks = 0, bke = 0, bvs = 0, bve = 0;
+        bool found = false;
+        for (;;) {
+            while (is_ws(p[i])) ++i;
+            if (p[i] == '}') break;
+            if (p[i] == ',') { ++i; while (is_ws(p[i])) ++i; }
+            const uint32_t ks = i;
+            i = (uint32_t)scan_string(p, i, e, f);
+            const uint32_t ke = i;
+            while (is_ws(p[i])) ++i;
+            ++i;                                   // ':'
+            while (is_ws(p[i])) ++i;
+            const uint32_t v0 = i;
+            i = (uint32_t)skip_value(p, i, e, f);
+            if (++members > PY_VALUE_MAX_MEMBERS) return -1;
+            if ((started & bit) && !key_less(p, lks[d], lke[d], ks + 1, ke - 1)) continue;   // emitted already
+            if (!found || !key_less(p, bks + 1, bke - 1, ks + 1, ke - 1)) { found = true; bks = ks; bke = ke; bvs = v0; bve = i; }
+        }
+        if (!found) { if (o) o[n] = '}'; ++n; --depth; continue; }
+        if (started & bit) { if (o) { o[n] = ','; o[n + 1] = ' '; } n += 2; }
+        started |= bit;
+        lks[d] = bks + 1; lke[d] = bke - 1;
+        n += o ? py_string_write(p, bks, bke, o + n) : py_string_len(p, bks, bke);
+        if (o) { o[n] = ':'; o[n + 1] = ' '; }
+        n += 2;
+        vs = bvs; ve = bve; have = true;
+    }
 }
 
 // Lane 0: classify args[0] for the handler and fill the record. `pr` is the parse of the payload.
@@ -86,7 +151,21 @@ __device__ inline void handler_phase_a(int handler, const uint8_t* __restrict__ 
             if (zero) return;
             rec.src_off = pr.a0_off; rec.src_len = pr.a0_len; rec.out_len = pr.a0_len; rec.mode = OM_COPY; rec.has = 1; return;
         }
-        default: rec.status = ST_UNSUPPORTED; return;                       // floats / non-empty containers
+        case AK_NUM: {
+            // any other number: its float64, as Python reads Go's text of it; +-0 (also by underflow) is falsy
+            unsigned long long b = 0;
+            if (!f64_parse(p, pr.a0_off, pr.a0_off + pr.a0_len, &b)) { rec.status = ST_UNSUPPORTED; return; }
+            if ((b << 1) == 0) return;
+            rec.value = (long long)b; rec.mode = OM_PY_NUM; rec.out_len = py_json_go_number(b, nullptr); rec.has = 1;
+            return;
+        }
+        case AK_ARR: case AK_OBJ: {                                          // non-empty: truthy
+            const int64_t n = py_value_json(p, pr.a0_off, pr.a0_off + pr.a0_len, nullptr);
+            if (n < 0) { rec.status = ST_UNSUPPORTED; return; }
+            rec.src_off = pr.a0_off; rec.src_len = pr.a0_len; rec.out_len = (uint32_t)n; rec.mode = OM_PY_VALUE; rec.has = 1;
+            return;
+        }
+        default: rec.status = ST_UNSUPPORTED; return;
         }
     }
     case 1: {   // crc32: zlib.crc32(s.encode()); a non-str has no .encode -> AttributeError
@@ -115,9 +194,16 @@ __device__ inline void handler_phase_a(int handler, const uint8_t* __restrict__ 
     }
     case 3: {   // json_sum: sum(obj["values"])
         if (pr.a0_kind != AK_OBJ) { rec.status = 1; return; }               // TypeError, or KeyError for {}
-        long long sum = 0;
-        int st = json_sum_object(p, pr.a0_off, pr.a0_off + pr.a0_len, &sum);
+        PySum ps;
+        int st = json_sum_object(p, pr.a0_off, pr.a0_off + pr.a0_len, &ps);
         if (st) { rec.status = (uint8_t)st; return; }
+        if (ps.is_float) {                                                  // 0.0 / -0.0 are falsy, NaN is not
+            const unsigned long long b = f64_to_bits(ps.f);
+            if ((b << 1) == 0) return;
+            rec.value = (long long)b; rec.mode = OM_PY_FLOAT; rec.out_len = py_json_float(b, nullptr); rec.has = 1;
+            return;
+        }
+        const long long sum = ps.i;
         if (sum == 0) return;
         rec.value = sum; rec.mode = OM_I64_DEC; rec.has = 1;
         rec.out_len = dec_len_u64((unsigned long long)(sum < 0 ? -sum : sum)) + (sum < 0 ? 1u : 0u);
@@ -128,18 +214,25 @@ __device__ inline void handler_phase_a(int handler, const uint8_t* __restrict__ 
     }
 }
 
-// phase B for the modes that are not plain copies: writes exactly rec.out_len bytes at o
+// phase B of the float64 and container modes, out of line (one call site in the kernels' main loops)
+__device__ __noinline__ void seq_emit_py(const uint8_t* __restrict__ p, const TaskRec& rec, uint8_t* __restrict__ o) {
+    if (rec.mode == OM_PY_NUM) py_json_go_number((unsigned long long)rec.value, o);
+    else if (rec.mode == OM_PY_FLOAT) py_json_float((unsigned long long)rec.value, o);
+    else py_value_json(p, rec.src_off, rec.src_off + rec.src_len, o);
+}
+
+// phase B for the modes that are not plain copies: writes exactly rec.out_len bytes at o. PY = false leaves out the
+// float64 / container modes (only identity's deferred tasks and json_sum make them), and with them a call in the other loops.
+template <bool PY = true>
 __device__ inline void seq_emit(const uint8_t* __restrict__ p, const TaskRec& rec, uint8_t* __restrict__ o) {
-    if (rec.mode == OM_VADD) vadd_write(p, rec.src_off, rec.src_len, o);
+    if (PY && rec.mode >= OM_PY_NUM) seq_emit_py(p, rec, o);
+    else if (rec.mode == OM_VADD) vadd_write(p, rec.src_off, rec.src_len, o);
     else if (rec.mode == OM_U32_DEC || rec.mode == OM_I64_DEC) {
         long long v = rec.value; uint32_t l = rec.out_len;
         if (v < 0) { *o++ = '-'; --l; v = -v; }
         write_dec(o, (unsigned long long)v, l);
     } else if (rec.mode == OM_STR_ESC) {                          // string the sequential parser sized (non-canonical frame)
-        uint32_t i = rec.src_off + 1, end = rec.src_off + rec.src_len - 1;
-        *o++ = '"';
-        while (i < end) o += py_emit(next_cp(p, i, end), o);
-        *o = '"';
+        py_string_write(p, rec.src_off, rec.src_off + rec.src_len, o);
     }
 }
 

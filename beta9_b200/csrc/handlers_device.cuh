@@ -8,6 +8,7 @@
 #pragma once
 #include <stdint.h>
 #include "json_device.cuh"
+#include "f64_device.cuh"
 
 namespace b9 {
 
@@ -50,7 +51,7 @@ __device__ inline uint32_t crc32_of_string_token(const uint8_t* __restrict__ p, 
 }
 
 // ---------------------------------------------------------------- json_sum (sum(obj["values"]))
-// status: 0 ok (value in *sum), 1 ERROR (KeyError / TypeError), 4 UNSUPPORTED (a float in the list)
+// status: 0 ok (value in *sum), 1 ERROR (KeyError / TypeError), 4 UNSUPPORTED (see sum_values_token)
 __device__ inline bool key_is_values(const uint8_t* __restrict__ p, uint32_t s, uint32_t e) {
     const char V[] = "values";
     uint32_t k = 0, i = s;
@@ -62,42 +63,103 @@ __device__ inline bool key_is_values(const uint8_t* __restrict__ p, uint32_t s, 
     return k == 6;
 }
 
-__device__ inline int sum_values_token(const uint8_t* __restrict__ p, uint32_t vs, uint32_t ve, long long* sum) {
-    // p[vs..ve) is a validated JSON value: the last "values" entry of the object
-    *sum = 0;
+// What Python's sum returns: an int until the first float term, a float from then on.
+struct PySum { long long i; double f; uint8_t is_float; };
+
+__device__ __forceinline__ double f64_add(double a, double b) {
+#ifdef __CUDA_ARCH__
+    return __dadd_rn(a, b);
+#else
+    return a + b;
+#endif
+}
+__device__ __forceinline__ double f64_abs(double a) { return f64_from_bits(f64_to_bits(a) & 0x7FFFFFFFFFFFFFFFull); }
+
+// Does Go write the finite double `bits` as digits only (so that json.loads makes a Python int of it)? Zero, and
+// integral values below 1e21.
+__device__ __forceinline__ bool go_text_is_int(unsigned long long bits) {
+    const unsigned long long mag = bits & 0x7FFFFFFFFFFFFFFFull;
+    if (mag == 0) return true;
+    const int bq = (int)(mag >> 52);
+    if (bq < 1023) return false;                                   // |x| < 1
+    if (bq < 1075 && (mag & ((1ull << (1075 - bq)) - 1ull))) return false;   // fraction bits
+    return f64_from_bits(mag) < 1e21;
+}
+
+// p[vs..ve) is a validated JSON value: the last "values" entry of the object. CPython >= 3.12's builtin sum over what
+// json.loads made of Go's text: ints (and bools) are added exactly in a C long while no float has come; the first float
+// converts the total and switches to float accumulation with Neumaier compensation, where float terms are compensated
+// and int terms are added as (double)value without compensation; the compensation is added at the end when it is
+// non-zero and finite (it would turn an infinite sum into NaN). DECLINED (4): a literal f64_parse cannot settle, and
+// an int outside the C long range (a term, or the running int total), where CPython leaves these loops for
+// arbitrary-precision arithmetic.
+__device__ __noinline__ int sum_values_token(const uint8_t* __restrict__ p, uint32_t vs, uint32_t ve, PySum* sum) {
+    sum->i = 0; sum->f = 0.0; sum->is_float = 0;
     uint8_t c = p[vs];
     if (c == '"') return (ve - vs == 2) ? 0 : 1;                  // sum("") == 0; sum("ab") raises
     if (c == '{') return only_ws(p, vs + 1, ve - 1) ? 0 : 1;      // sum({}) == 0; str keys raise
     if (c != '[') return 1;                                        // not iterable
     uint32_t i = vs + 1;
-    long long acc = 0; bool unsupported = false;
+    long long acc = 0; double fs = 0.0, comp = 0.0; bool fl = false, unsupported = false;
     while (i < ve && is_ws(p[i])) ++i;
     if (p[i] == ']') return 0;
     for (;;) {
         uint8_t d = p[i];
+        bool is_int = true; long long iv = 0; double fv = 0.0;
         if (d == '-' || is_digit(d)) {
             uint32_t f = 0; bool simple = false;
             int64_t e = scan_number(p, i, ve, f, &simple);
-            if (simple) {
+            if (simple) {                                          // <= 15 digits: exact in a float64, Go writes them back
                 bool neg = d == '-'; long long v = 0;
                 for (uint32_t k = i + (neg ? 1 : 0); k < (uint32_t)e; ++k) v = v * 10 + (p[k] - '0');
-                acc += neg ? -v : v;
-            } else unsupported = true;                              // needs float64 arithmetic / repr
+                iv = neg ? -v : v;
+            } else {
+                unsigned long long b = 0;
+                if (!f64_parse(p, i, (uint32_t)e, &b)) unsupported = true;
+                else if (go_text_is_int(b)) {
+                    // the int is the value of Go's text: the shortest digits padded with zeros (2^55 - 2 reads as
+                    // 36028797018963970, not 36028797018963966)
+                    const F64Dec dd = f64_shortest(b);
+                    unsigned long long m = dd.f;
+                    const unsigned long long lim = dd.neg ? 9223372036854775808ull : 9223372036854775807ull;
+                    for (int z = dd.n; z < dd.dp && m <= lim; ++z) m = (m > lim / 10u) ? lim + 1u : m * 10u;
+                    if (dd.cls == 1) iv = 0;
+                    else if (m <= lim) iv = dd.neg ? (long long)(0ull - m) : (long long)m;
+                    else unsupported = true;
+                } else { is_int = false; fv = f64_from_bits(b); }
+            }
             i = (uint32_t)e;
-        } else if (d == 't') { acc += 1; i += 4; }                 // True + 1 == 2
+        } else if (d == 't') { iv = 1; i += 4; }                   // True + 1 == 2
         else if (d == 'f') { i += 5; }
         else return 1;                                             // None / str / list / dict: TypeError
+        if (!unsupported) {
+            if (!fl) {
+                if (is_int) {
+                    if (acc >= 0 ? (iv <= 9223372036854775807ll - acc) : (iv >= (-9223372036854775807ll - 1) - acc)) acc += iv;
+                    else unsupported = true;
+                } else { fs = f64_add((double)acc, fv); comp = 0.0; fl = true; }
+            } else if (is_int) fs = f64_add(fs, (double)iv);
+            else {
+                const double t = f64_add(fs, fv);
+                if (f64_abs(fs) >= f64_abs(fv)) comp = f64_add(comp, f64_add(f64_add(fs, -t), fv));
+                else comp = f64_add(comp, f64_add(f64_add(fv, -t), fs));
+                fs = t;
+            }
+        }
         while (i < ve && is_ws(p[i])) ++i;
         if (p[i] == ',') { ++i; while (i < ve && is_ws(p[i])) ++i; continue; }
         break;                                                     // ']'
     }
     if (unsupported) return 4;
-    *sum = acc;
+    if (fl) {
+        if (comp != 0.0 && (f64_to_bits(comp) & 0x7FF0000000000000ull) != 0x7FF0000000000000ull) fs = f64_add(fs, comp);
+        sum->f = fs; sum->is_float = 1;
+    } else sum->i = acc;
     return 0;
 }
 
 // arg token p[s..e) is a non-empty object (validated). Finds the last "values" key.
-__device__ inline int json_sum_object(const uint8_t* __restrict__ p, uint32_t s, uint32_t e, long long* sum) {
+__device__ inline int json_sum_object(const uint8_t* __restrict__ p, uint32_t s, uint32_t e, PySum* sum) {
     uint32_t i = s + 1;
     bool found = false; uint32_t vs = 0, ve = 0;
     for (;;) {

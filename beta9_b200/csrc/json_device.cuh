@@ -278,6 +278,17 @@ __device__ inline uint32_t next_cp(const uint8_t* __restrict__ p, uint32_t& i, u
     return 0xFFFDu;
 }
 
+// decoded keys a (body p[as..ae)) < b, bytewise on their UTF-8 (== code point order): the order Go's encoder
+// writes map keys in
+__device__ inline bool key_less(const uint8_t* __restrict__ p, uint32_t as, uint32_t ae, uint32_t bs, uint32_t be) {
+    uint32_t i = as, j = bs;
+    while (i < ae && j < be) {
+        uint32_t a = next_cp(p, i, ae), b = next_cp(p, j, be);
+        if (a != b) return a < b;
+    }
+    return i >= ae && j < be;
+}
+
 // encoding/json struct-key matching for TaskPayload: 1 = "args", 2 = "kwargs", 0 = neither.
 // Exact match or equal under foldName (ASCII case, U+212A -> k, U+017F -> s). body = p[s..e).
 __device__ inline int match_payload_key(const uint8_t* __restrict__ p, uint32_t s, uint32_t e) {

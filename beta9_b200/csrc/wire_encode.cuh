@@ -54,16 +54,6 @@ __device__ inline uint32_t go_emit(uint32_t cp, uint8_t* __restrict__ o) {
     o[0] = 0xF0 | (cp >> 18); o[1] = 0x80 | ((cp >> 12) & 0x3F); o[2] = 0x80 | ((cp >> 6) & 0x3F); o[3] = 0x80 | (cp & 0x3F); return 4;
 }
 
-// decoded keys a (body p[as..ae)) < b, bytewise on their UTF-8 (== code point order)
-__device__ inline bool key_less(const uint8_t* __restrict__ p, uint32_t as, uint32_t ae, uint32_t bs, uint32_t be) {
-    uint32_t i = as, j = bs;
-    while (i < ae && j < be) {
-        uint32_t a = next_cp(p, i, ae), b = next_cp(p, j, be);
-        if (a != b) return a < b;
-    }
-    return i >= ae && j < be;
-}
-
 // Re-encode the validated JSON value p[s..e) by Go's rules. o == nullptr: size only.
 // Returns the byte count, or -1 if the value is outside the device domain.
 __device__ inline int64_t go_transcode(const uint8_t* __restrict__ p, uint32_t s, uint32_t e, uint8_t* __restrict__ o) {

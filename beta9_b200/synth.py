@@ -242,6 +242,82 @@ def json_batch(n: int, doc_bytes: int = 1024, seed: int = SEED, name: str = "jso
     return _pack(chunks, lens, task_ids(n, seed), name)
 
 
+def _float_value(rng: np.random.Generator):
+    """One number of json_float_batch: short decimals, 17-digit values, subnormals, values >= 1e21, integers above 2^53,
+    small integers."""
+    k = int(rng.integers(0, 8))
+    if k == 0:
+        return round(float(rng.uniform(-1000, 1000)), int(rng.integers(0, 4)))     # 12.5, -0.37, 401.0
+    if k == 1:
+        return float(rng.uniform(-1, 1)) * 10.0 ** int(rng.integers(-8, 9))          # 16-17 digits
+    if k == 2:
+        return float(np.uint64(rng.integers(1, 1 << 52)).view(np.float64)) * (1 if rng.random() < 0.5 else -1)   # subnormal
+    if k == 3:
+        return float(rng.uniform(1, 10)) * 10.0 ** int(rng.integers(21, 300))       # >= 1e21
+    if k == 4:
+        return int(rng.integers(1 << 53, 1 << 57)) * (1 if rng.random() < 0.7 else -1)   # above 2^53; sums stay in a C long
+    if k == 5:
+        return float(rng.integers(-10**6, 10**6))                                  # integral floats: 7.0
+    return int(rng.integers(0, 10**6))
+
+
+def json_float_batch(n: int, doc_bytes: int = 1024, seed: int = SEED, name: str = "json_sum_f64") -> Batch:
+    """configs[4]'s document shape `{"id": i, "values": [...], "pad": "xxx"}` with float64 values (see _float_value),
+    about `doc_bytes` of JSON text each."""
+    rng = np.random.default_rng(seed + 5)
+    chunks: List[bytes] = []
+    lens = np.empty(n, dtype=np.uint64)
+    for i in range(n):
+        vals = []
+        doc = {"id": i, "values": vals, "pad": ""}
+        cur = len(json.dumps(doc))
+        while cur < doc_bytes - 40:
+            vals.append(_float_value(rng))
+            cur += len(json.dumps(vals[-1])) + (2 if len(vals) > 1 else 0)
+        doc["pad"] = "x" * max(0, doc_bytes - cur)
+        b = json.dumps({"args": (doc,), "kwargs": {}}).encode("utf-8")
+        chunks.append(b)
+        lens[i] = len(b)
+    return _pack(chunks, lens, task_ids(n, seed), name)
+
+
+_VALUE_STRINGS = ["", "a", "abc", "café", "<tag>", "line\nbreak", "q\"uote", "\U0001f600", " ", "tab\t", "back\\slash", "key"]
+
+
+def _sdk_value(rng: np.random.Generator, depth: int):
+    k = int(rng.integers(0, 10 if depth < 4 else 6))
+    if k == 0:
+        return bool(rng.random() < 0.5)
+    if k == 1:
+        return None if rng.random() < 0.3 else int(rng.integers(-10**6, 10**6))
+    if k == 2:
+        return _float_value(rng)
+    if k in (3, 4):
+        return _VALUE_STRINGS[int(rng.integers(0, len(_VALUE_STRINGS)))] + str(int(rng.integers(0, 100)))
+    if k == 5:
+        return round(float(rng.uniform(-100, 100)), int(rng.integers(0, 6)))
+    if k in (6, 7):
+        return [_sdk_value(rng, depth + 1) for _ in range(int(rng.integers(0, 6)))]
+    keys = ["id", "name", "value", "a", "b", "x", "été", "Z", "items", "k" + str(int(rng.integers(0, 9)))]
+    return {keys[int(j)]: _sdk_value(rng, depth + 1) for j in rng.integers(0, len(keys), size=int(rng.integers(0, 7)))}
+
+
+def values_batch(n: int, seed: int = SEED, name: str = "identity_values") -> Batch:
+    """SDK payloads `json.dumps({"args": (v,), "kwargs": {}})` of random nested lists and dicts (and some bare numbers)
+    holding numbers, strings, booleans and None."""
+    rng = np.random.default_rng(seed + 6)
+    chunks: List[bytes] = []
+    lens = np.empty(n, dtype=np.uint64)
+    for i in range(n):
+        r = rng.random()
+        v = _float_value(rng) if r < 0.1 else ([_sdk_value(rng, 1) for _ in range(int(rng.integers(1, 8)))] if r < 0.55 else
+                                                 {"id": i, "data": _sdk_value(rng, 1), "tags": [_sdk_value(rng, 2) for _ in range(3)]})
+        b = json.dumps({"args": (v,), "kwargs": {}}).encode("utf-8")
+        chunks.append(b)
+        lens[i] = len(b)
+    return _pack(chunks, lens, task_ids(n, seed), name)
+
+
 def concat(batches: List[Batch]) -> Batch:
     ids = np.concatenate([b.task_ids for b in batches])
     payload = np.concatenate([b.payload for b in batches])

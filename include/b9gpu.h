@@ -54,10 +54,13 @@ extern "C" {
  *      for which a device implementation exists. Semantics are those of the Python functions in
  *      oracle/pyoracle/handlers.py invoked as `handler(*args, **kwargs)`. ------------------- */
 enum b9_handler {
-    B9_H_IDENTITY = 0,  /* def identity(s, /): return s              (configs[0] echo, configs[1])   */
+    B9_H_IDENTITY = 0,  /* def identity(s, /): return s              (configs[0] echo, configs[1])
+                         * any JSON argument: strings, numbers (float64, Python's int/float reading of
+                         * Go's text), non-empty lists and objects (Go's sorted, de-duplicated keys)     */
     B9_H_CRC32    = 1,  /* def crc32(s, /): return zlib.crc32(s.encode())                (configs[2]) */
     B9_H_VADD_F32 = 2,  /* base64(fp32 a||b) -> base64(a+b)                               (configs[3]) */
-    B9_H_JSON_SUM = 3,  /* def json_sum(obj, /): return sum(obj["values"])                (configs[4]) */
+    B9_H_JSON_SUM = 3,  /* def json_sum(obj, /): return sum(obj["values"])                (configs[4])
+                         * ints exactly in a C long, floats with CPython 3.12's compensated sum       */
     B9_H_COUNT_
 };
 
@@ -67,8 +70,11 @@ enum b9_handler {
  * answered TaskQueuePutResponse{Ok:false} and never created the task
  * (pkg/abstractions/taskqueue/taskqueue.go:213-218): the batch interface validates on the device,
  * at drain time. UNSUPPORTED means the payload is valid but outside what the device handler
- * implements (e.g. a float that needs shortest-repr formatting): the host must route that task
- * through the reference's own CPU loop. The device never guesses. */
+ * implements: the host must route that task through the reference's own CPU loop. The device
+ * never guesses. For identity and json_sum that is: a number literal of more than 19 significant
+ * digits whose rounding the fast parser cannot settle, nesting deeper than 16 (identity) / 64
+ * levels, an object of more than 64 members (identity), and a json_sum whose Python value needs
+ * an int outside the C long range. */
 enum b9_status {
     B9_ST_COMPLETE    = 0,
     B9_ST_ERROR       = 1,
