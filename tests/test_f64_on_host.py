@@ -8,14 +8,13 @@ import ctypes as C
 import json
 import math
 import os
-import struct
 import subprocess
-from fractions import Fraction
 
 import numpy as np
 import pytest
 
 from oracle.pyoracle.gojson import go_format_float64
+from tests.f64_corpus import _bits, _literals, _patterns, _powers, _sig_digits
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(HERE, "host_shim", "f64_shim.cpp")
@@ -60,60 +59,6 @@ def f64():
     return F64
 
 
-def _bits(x: float) -> int:
-    return struct.unpack("<Q", struct.pack("<d", x))[0]
-
-
-def _sig_digits(lit: str) -> int:
-    m = lit.lstrip("-").split("e")[0].split("E")[0].replace(".", "").lstrip("0")
-    return len(m)
-
-
-def _literals():
-    rng = np.random.default_rng(20261015)
-    pats = rng.integers(0, 1 << 64, size=280_000, dtype=np.uint64)
-    xs = [x for x in pats.view(np.float64).tolist() if math.isfinite(x)]
-    out = []
-    for x in xs:
-        out += [repr(x), "%.17g" % x, "%.25e" % x]
-    specials = [5e-324, 1e-323, 2.2250738585072009e-308, 2.2250738585072014e-308, 1.7976931348623157e308, 2.0 ** 53 - 1, 2.0 ** 53,
-                2.0 ** 53 + 2, 1e22, 1e23, 0.1, 0.3, 1.5, 123.0, 1e20, 1e21, 1e-7]
-    for x in specials:
-        out += [repr(x), "%.17g" % x, "%.25e" % x, "%.40e" % x]
-    out += ["9007199254740993", "9007199254740991", "9007199254740992", "1e22", "1e23", "8.98846567431158e307", "0", "-0", "0.0", "-0.0",
-            "1e400", "-1e400", "1e-400", "-1e-400", "1e-350", "1e-342", "1e-343", "1e308", "1e309", "1.7976931348623158e308",
-            "1.7976931348623159e308", "179769313486231580793728971405303415079934132710037826936173778980444968292764750946649017977587207096330286416692887910946555547851940402630657488671505820681908902000708383676273854845817711531764475730270069855571366959622842914819860834936475292719074168444365510704342711559699508093042880177904174497791",
-            "2.4703282292062327e-324", "2.4703282292062328e-324", "4.9406564584124654e-324", "1e-5", "0.000001", "0." + "0" * 300 + "1",
-            "1" + "0" * 300, "00", "1.00000000000000000000000000000000000000000"]
-    out = [s for s in out if not s.startswith("00")]
-    for _ in range(60_000):                                 # 1..19 digits, exponents -400..400
-        nd = int(rng.integers(1, 20))
-        w = "".join(map(str, rng.integers(0, 10, size=nd).tolist())).lstrip("0") or "1"
-        out.append("%se%d" % (w, int(rng.integers(-400, 401))))
-    # subnormals
-    sub = rng.integers(1, 1 << 52, size=20_000, dtype=np.uint64).view(np.float64).tolist()
-    out += [repr(x) for x in sub] + ["%.17g" % x for x in sub]
-    # 20-40 digit literals at exact midpoints between adjacent doubles, and one unit of the last digit either side
-    for _ in range(40_000):
-        m = int(rng.integers(1 << 52, 1 << 53))
-        if rng.random() < 0.5:
-            e = int(rng.integers(11, 72))                   # integers: (2m+1) 2^(e-1)
-            mid = Fraction((2 * m + 1) << (e - 1))
-        else:
-            j = int(rng.integers(1, 23))                    # fractions with j+1 decimals: (2m+1) 2^-(j+1)
-            mid = Fraction(2 * m + 1, 1 << (j + 1))
-        den_pow = 0
-        while (mid * 10 ** den_pow).denominator != 1:
-            den_pow += 1
-        digits = str((mid * 10 ** den_pow).numerator)
-        for delta in (0, -1, 1):
-            d = str(int(digits) + delta)
-            lit = d + "e-%d" % den_pow if den_pow else d
-            if 20 <= _sig_digits(lit) <= 40:
-                out.append(("-" if rng.random() < 0.3 else "") + lit)
-    return out
-
-
 def test_parser_against_float(f64):
     lits = _literals()
     assert len(lits) >= 1_000_000
@@ -129,21 +74,6 @@ def test_parser_against_float(f64):
         assert b == _bits(want), (lit, hex(b), want)
     n_long = sum(1 for s in lits if _sig_digits(s) > 19)
     print(f"\nf64_parse: {len(lits)} literals, {n_long} with > 19 significant digits, {declined_long} of those declined")
-
-
-def _patterns(n: int, seed: int):
-    rng = np.random.default_rng(seed)
-    b = rng.integers(0, 1 << 64, size=n, dtype=np.uint64)
-    return b[(b & np.uint64(0x7FF0000000000000)) != np.uint64(0x7FF0000000000000)]
-
-
-def _powers():
-    xs = [2.0 ** e for e in range(-1074, 1024)] + [float("1e%d" % e) for e in range(-323, 309)]
-    xs += [5e-324 * k for k in range(1, 50)] + [1.7976931348623157e308, 2.2250738585072014e-308, 1e21, 1e-6, 1e16, 1e-4, 1e-5]
-    xs += [math.nextafter(x, math.inf) for x in list(xs)] + [math.nextafter(x, 0.0) for x in list(xs)]
-    xs = [x for x in xs if math.isfinite(x)]
-    xs += [-x for x in xs] + [0.0, -0.0]
-    return np.array([_bits(x) for x in xs], dtype=np.uint64)
 
 
 def _py_float_json(x: float) -> str:
