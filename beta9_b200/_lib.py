@@ -12,6 +12,7 @@ B9_OK, B9_EINVAL, B9_ENOMEM, B9_ENOSPC, B9_E2BIG, B9_EIO, B9_ENODEV, B9_ENOSYS, 
 H_IDENTITY, H_CRC32, H_VADD_F32, H_JSON_SUM = 0, 1, 2, 3
 ST_COMPLETE, ST_ERROR, ST_RETRY, ST_REJECTED, ST_UNSUPPORTED = 0, 1, 2, 3, 4
 TF_CANCELLED = 0x01
+TF_HTTP_BODY, TF_PICKLE, TF_TASK_MSG = 0x02, 0x04, 0x08
 
 
 class Opts(C.Structure):

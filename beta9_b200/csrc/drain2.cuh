@@ -29,6 +29,7 @@
 #include <type_traits>
 #include "drain_kernel.cuh"
 #include "vadd_fast.cuh"
+#include "task_msg.cuh"
 
 namespace b9 {
 
@@ -485,7 +486,8 @@ __device__ __forceinline__ bool crc_scan_coop(LD ld, const uint8_t* __restrict__
     return true;
 }
 
-template <int HANDLER> __device__ __noinline__ void d2_parse_and_size(const uint8_t* p, uint32_t len, TaskRec& rec, const uint32_t* crc_table, bool http = false);
+template <int HANDLER> __device__ __noinline__ void d2_parse_and_size(const uint8_t* p, uint32_t len, TaskRec& rec, const uint32_t* crc_table, bool http = false,
+                                                                      const uint4* rec_id = nullptr);
 // one crc32 task with the whole warp; the owner lane keeps the record. `in_smem`: p points into this warp's stage buffer.
 __device__ __forceinline__ void crc_task_coop(const uint8_t* __restrict__ p, bool in_smem, uint32_t len, int lane, bool owner, const uint32_t* crc_table,
                                               const uint32_t* __restrict__ shift_tabs, TaskRec& rec) {
@@ -899,10 +901,20 @@ template <int HANDLER>
 __device__ __forceinline__ void d2_phase_b_task(const uint8_t* __restrict__ p, const TaskRec& rec, uint8_t* __restrict__ o) { seq_emit<HANDLER == 3>(p, rec, o); }
 
 // the sequential validating parser + handler sizing, out of line: rare for identity, and it keeps the
-// hot loops' registers and instruction-cache footprint small
+// hot loops' registers and instruction-cache footprint small. record: the bytes are a TaskMessage record
+// (B9_TF_TASK_MSG) of the task whose 16-byte id is *rec_id (global memory); together with the HTTP-body flag it is not answered.
 template <int HANDLER>
-__device__ __noinline__ void d2_parse_and_size(const uint8_t* p, uint32_t len, TaskRec& rec, const uint32_t* crc_table, bool http) {
-    Parsed pr = parse_payload(p, len, http);
+__device__ __noinline__ void d2_parse_and_size(const uint8_t* p, uint32_t len, TaskRec& rec, const uint32_t* crc_table, bool http,
+                                               const uint4* rec_id) {
+    Parsed pr;
+    if (rec_id) {
+        uint8_t idb[16];
+        const uint4 id = __ldcg(rec_id);
+        const uint32_t w[4] = {id.x, id.y, id.z, id.w};
+        for (int b = 0; b < 16; ++b) idb[b] = (uint8_t)(w[b >> 2] >> (8 * (b & 3)));
+        pr = parse_task_msg(p, len, idb);
+        if (http) pr.status = ST_UNSUPPORTED;
+    } else pr = parse_payload(p, len, http);
     handler_phase_a(HANDLER, p, pr, rec, crc_table);
 }
 
@@ -1134,6 +1146,103 @@ __device__ __noinline__ bool esc_verify_canonical(uint8_t* __restrict__ sbuf, ui
     return carry == 0u;
 }
 
+// ------------------------------------------------------------------ identity: TaskMessage records, settled in the main loop
+// TaskMessage.Encode (pkg/types/task.go:79-90) writes one fixed shape:
+//   {"task_id":"<36>","workspace_name":"…","stub_id":"…","executor":"…","args":["<body>"],"kwargs":{}|null,
+//    "policy":{"max_retries":D,"timeout":D,"expires":"…","ttl":D},"retries":D,"timestamp":D}
+// One thread per record matches it: the head from the front (the id text against the slot's id), the envelope strings
+// as plain ASCII, the policy tail from the BACK -- a regular grammar without escapes, so the body's span comes out
+// without a walk over the body's escapes. Everything here is inside the domain of task_msg.cuh, and the answer is the
+// one parse_task_msg + handler_phase_a would give.
+// p[i, ...) is the body of a plain-ASCII string (no '\\', no controls, nothing >= 0x7F): the index of its closing quote, or 0
+__device__ __forceinline__ uint32_t tm_plain_string_end(const uint8_t* __restrict__ p, uint32_t i, uint32_t n) {
+    while (i < n) {                                                        // (reads up to 3 bytes past n: stage buffer slack)
+        const uint32_t m = special_mask32(ld_u32_unaligned(p + i));
+        if (!m) { i += 4; continue; }
+        const uint32_t j = i + ((uint32_t)(__ffs(m) - 1) >> 3);
+        return (j < n && p[j] == '"') ? j : 0u;
+    }
+    return 0u;
+}
+// p[j - k, j) == lit: moves j to its start
+__device__ __forceinline__ bool tm_back_lit(const uint8_t* __restrict__ p, uint32_t& j, const char* lit, uint32_t k) {
+    if (j < k) return false;
+    for (uint32_t t = 0; t < k; ++t) if (p[j - k + t] != (uint8_t)lit[t]) return false;
+    j -= k;
+    return true;
+}
+// a JSON integer of at most 20 digits ends at j: moves j to its start
+__device__ __forceinline__ bool tm_back_int(const uint8_t* __restrict__ p, uint32_t& j) {
+    const uint32_t e = j;
+    while (j > 0 && e - j <= 20u && is_digit(p[j - 1])) --j;
+    const uint32_t nd = e - j;
+    if (nd == 0 || nd > 20u || (nd > 1 && p[j] == '0')) return false;
+    if (j > 0 && p[j - 1] == '-') --j;
+    return true;
+}
+// 0: not this shape (the kernel's tail decides). Otherwise the string token of args[0]: its start | its length << 32, and
+// bit 63 when the body holds escapes -- then esc_verify_canonical decides. A body with a surrogate escape, a control byte,
+// DEL or non-ASCII is left to the tail: Python keeps lone surrogates, and json.dumps escapes the others.
+__device__ __noinline__ unsigned long long task_msg_quick(const uint8_t* __restrict__ p, uint32_t n, const uint4* __restrict__ idp) {
+    if (n < 128u || p[n - 1] != '}') return 0ull;
+    // ---- the head
+    uint32_t i = 12u;
+    if (!tm_back_lit(p, i, "{\"task_id\":\"", 12u)) return 0ull;
+    {
+        const uint4 id = __ldg(idp);
+        const uint32_t w[4] = {id.x, id.y, id.z, id.w};
+        uint32_t k = 12u;
+        for (int b = 0; b < 16; ++b) {
+            if (b == 4 || b == 6 || b == 8 || b == 10) { if (p[k] != '-') return 0ull; ++k; }
+            const uint32_t v = (w[b >> 2] >> (8 * (b & 3))) & 0xFFu;
+            if (p[k] != hexdig(v >> 4) || p[k + 1] != hexdig(v & 15u)) return 0ull;
+            k += 2;
+        }
+    }
+    i = 68u;
+    if (!tm_back_lit(p, i, "\",\"workspace_name\":\"", 20u)) return 0ull;
+    i = tm_plain_string_end(p, 68u, n);
+    if (!i || i + 13u > n) return 0ull;
+    { uint32_t j = i + 13u; if (!tm_back_lit(p, j, "\",\"stub_id\":\"", 13u)) return 0ull; }
+    i = tm_plain_string_end(p, i + 13u, n);
+    if (!i || i + 14u > n) return 0ull;
+    { uint32_t j = i + 14u; if (!tm_back_lit(p, j, "\",\"executor\":\"", 14u)) return 0ull; }
+    i = tm_plain_string_end(p, i + 14u, n);
+    if (!i || i + 11u > n) return 0ull;
+    { uint32_t j = i + 11u; if (!tm_back_lit(p, j, "\",\"args\":[\"", 11u)) return 0ull; }
+    const uint32_t bs = i + 11u;                                           // first byte of the body
+    // ---- the tail, from the back
+    uint32_t j = n - 1;
+    if (!tm_back_int(p, j) || !tm_back_lit(p, j, ",\"timestamp\":", 13u)) return 0ull;
+    if (!tm_back_int(p, j) || !tm_back_lit(p, j, ",\"retries\":", 11u)) return 0ull;
+    if (!tm_back_lit(p, j, "}", 1u) || !tm_back_int(p, j) || !tm_back_lit(p, j, "\",\"ttl\":", 8u)) return 0ull;
+    while (j > bs && p[j - 1] != '"' && !byte_special(p[j - 1])) --j;     // expires: plain ASCII
+    if (!tm_back_lit(p, j, ",\"expires\":\"", 12u)) return 0ull;
+    if (!tm_back_int(p, j) || !tm_back_lit(p, j, ",\"timeout\":", 11u)) return 0ull;
+    if (!tm_back_int(p, j) || !tm_back_lit(p, j, ",\"policy\":{\"max_retries\":", 25u)) return 0ull;
+    if (!tm_back_lit(p, j, ",\"kwargs\":{}", 12u) && !tm_back_lit(p, j, ",\"kwargs\":null", 14u)) return 0ull;
+    if (!tm_back_lit(p, j, "\"]", 2u) || j < bs) return 0ull;
+    const uint32_t be = j;                                                 // the body's closing quote
+    // ---- the body: plain, or escapes to verify
+    uint32_t sp = 0;
+    uint32_t k = bs;
+    for (; k + 4u <= be; k += 4u) sp |= special_mask32(ld_u32_unaligned(p + k));
+    for (; k < be; ++k) sp |= byte_special(p[k]) ? 1u : 0u;
+    const unsigned long long tok = (unsigned long long)(bs - 1u) | ((unsigned long long)(be - bs + 2u) << 32);
+    if (!sp) return tok;
+    for (k = bs; k < be; ++k) {
+        const uint32_t c = p[k];
+        if (c < 0x20u || c >= 0x7Fu || c == '"') return 0ull;
+        if (c == '\\') {
+            if (k + 1u >= be) return 0ull;                                 // the closing quote would be escaped
+            if (p[k + 1] == 'u' && k + 3u < be && p[k + 2] == 'd' && ((p[k + 3] >= '8' && p[k + 3] <= '9') || (p[k + 3] >= 'a' && p[k + 3] <= 'f')))
+                return 0ull;
+            ++k;
+        }
+    }
+    return tok | (1ull << 63);
+}
+
 // ------------------------------------------------------------------ cloudpickle-framed tasks (the function path)
 // `Function.map()` sends cloudpickle.dumps({"args": args, "kwargs": kwargs}) per input (sdk/src/beta9/abstractions/function.py:
 // 198-205,246-262); the gateway hands a blob that starts 80 05 95 to the runner as it is (pkg/abstractions/function/task.go:
@@ -1170,29 +1279,7 @@ __device__ __forceinline__ bool range_has_high_bit(const uint8_t* __restrict__ p
     for (; i < hi; ++i) acc |= p[i];
     return (acc & 0x80808080u) != 0u;
 }
-// UTF-8 as Python decodes a pickled str ("surrogatepass": the 3-byte encodings of U+D800..DFFF are accepted)
-__device__ __noinline__ bool utf8_valid_surrogatepass(const uint8_t* __restrict__ b, uint32_t n) {
-    uint32_t i = 0;
-    while (i < n) {
-        const uint8_t c = b[i];
-        if (c < 0x80) { ++i; continue; }
-        if (c >= 0xC2 && c <= 0xDF) { if (i + 2 > n || (b[i + 1] & 0xC0) != 0x80) return false; i += 2; continue; }
-        if (c >= 0xE0 && c <= 0xEF) {
-            if (i + 3 > n) return false;
-            const uint8_t lo = c == 0xE0 ? 0xA0 : 0x80;
-            if (b[i + 1] < lo || b[i + 1] > 0xBF || (b[i + 2] & 0xC0) != 0x80) return false;
-            i += 3; continue;
-        }
-        if (c >= 0xF0 && c <= 0xF4) {
-            if (i + 4 > n) return false;
-            const uint8_t lo = c == 0xF0 ? 0x90 : 0x80, hi = c == 0xF4 ? 0x8F : 0xBF;
-            if (b[i + 1] < lo || b[i + 1] > hi || (b[i + 2] & 0xC0) != 0x80 || (b[i + 3] & 0xC0) != 0x80) return false;
-            i += 4; continue;
-        }
-        return false;
-    }
-    return true;
-}
+// (a pickled str's UTF-8 is checked by utf8_valid_surrogatepass, task_msg.cuh)
 __device__ __forceinline__ void pickle_result_header(uint8_t* __restrict__ o, uint32_t frame_len) {    // 80 05 95 <u64>
     o[0] = 0x80; o[1] = 0x05; o[2] = 0x95;
     o[3] = (uint8_t)frame_len; o[4] = (uint8_t)(frame_len >> 8); o[5] = (uint8_t)(frame_len >> 16); o[6] = (uint8_t)(frame_len >> 24);
@@ -1206,7 +1293,8 @@ __device__ __forceinline__ void pickle_result_header(uint8_t* __restrict__ o, ui
 // empty for SDK-made payloads, and a second launch cost every drain a kernel boundary for nothing.)
 // No worker ever waits for another one: a worker takes what is claimable and leaves; every worker publishes its items
 // BEFORE it counts itself done, so the worker that counts last sees the final list and drains what is left.
-__device__ __noinline__ void slow_task(const DrainArgs& a, uint64_t goff, uint32_t lenw, uint32_t j, bool pickle, uint8_t* __restrict__ stage, uint32_t stage_cap, int lane) {
+__device__ __noinline__ void slow_task(const DrainArgs& a, uint64_t goff, uint32_t lenw, uint32_t j, bool pickle, bool record, uint8_t* __restrict__ stage,
+                                       uint32_t stage_cap, int lane) {
     const uint32_t len = lenw & 0x3FFFFFFFu;
     const bool http = (lenw & 0x40000000u) != 0;
     const uint8_t* p = a.payload + goff;
@@ -1254,7 +1342,10 @@ __device__ __noinline__ void slow_task(const DrainArgs& a, uint64_t goff, uint32
         if (par) { rec.has = 1; rec.mode = OM_STR_PAR; rec.src_off = FRAME_PRE_LEN; rec.src_len = nbody; rec.out_len = ol; }
     }
     if (!par) {                                                            // the sequential validating parser decides
-        if (lane == 0) d2_parse_and_size<0>(p, len, rec, nullptr, http);
+        if (lane == 0) {
+            // a TaskMessage record: its id is the one the main loop wrote to the record (before it published the item)
+            d2_parse_and_size<0>(p, len, rec, nullptr, http, record ? a.out_ids + j : nullptr);
+        }
         rec.src_off = __shfl_sync(0xffffffffu, rec.src_off, 0); rec.src_len = __shfl_sync(0xffffffffu, rec.src_len, 0);
         rec.out_len = __shfl_sync(0xffffffffu, rec.out_len, 0);
         const uint32_t w = __shfl_sync(0xffffffffu, (uint32_t)rec.status | ((uint32_t)rec.has << 8) | ((uint32_t)rec.mode << 16), 0);
@@ -1313,7 +1404,8 @@ __device__ __noinline__ void d3_identity_tail(const DrainArgs& a, uint8_t* __res
             w1 = *(const volatile unsigned long long*)&a.slow[i].w1;
         }
         w0 = __shfl_sync(0xffffffffu, w0, 0); w1 = __shfl_sync(0xffffffffu, w1, 0);
-        slow_task(a, w0 & ((1ull << 40) - 1ull), (uint32_t)w1, (uint32_t)(w1 >> 32) & 0xFFFFFFu, ((w1 >> 56) & 1ull) != 0ull, stage, stage_cap, lane);
+        slow_task(a, w0 & ((1ull << 40) - 1ull), (uint32_t)w1, (uint32_t)(w1 >> 32) & 0xFFFFFFu, ((w1 >> 56) & 1ull) != 0ull, ((w1 >> 57) & 1ull) != 0ull,
+                  stage, stage_cap, lane);
     }
 }
 
@@ -1455,6 +1547,10 @@ __global__ void __launch_bounds__(D3_WARPS * 32, (HANDLER == 1 ? B9_CRC_MINB : H
                         }
                     }
                 }
+                if (W.flg[k] & B9_TF_TASK_MSG_BIT) {                       // a TaskMessage record: the kernel's tail, unless the check below settles it
+                    rec.has = 0; rec.out_len = 0; rec.mode = OM_DEFER; rec.value = 3;
+                    if (my_http || my_pickle) { rec.mode = OM_NONE; rec.value = 0; rec.status = ST_UNSUPPORTED; }   // no record is either
+                }
             }
             if constexpr (HANDLER == 0 && T == 32) {
                 // framed, but the body holds escapes: the warp checks that they are json.dumps's own (then the task is a copy after all)
@@ -1469,14 +1565,40 @@ __global__ void __launch_bounds__(D3_WARPS * 32, (HANDLER == 1 ? B9_CRC_MINB : H
                         rec.has = 1; rec.mode = OM_COPY; rec.src_off = FRAME_PRE_LEN - 1; rec.src_len = tok; rec.out_len = tok; rec.value = 0;
                     }
                 }
+                // TaskMessage records (B9_TF_TASK_MSG), only on tiles that hold one: Go's fixed shape with a clean body is a copy
+                // of the token, a body with escapes is a copy when they are json.dumps's own; the rest goes to the tail
+                const bool my_rec = mine && rec.mode == OM_DEFER && rec.value == 3;
+                if (__any_sync(0xffffffffu, my_rec)) {
+                    unsigned long long qm = 0;
+                    if (my_rec && staged) qm = task_msg_quick(sbuf + my_soff, my_len, a.ids + ((a.first_task + t0 + k) & a.slot_mask));
+                    const uint32_t ts = (uint32_t)qm, tl = (uint32_t)(qm >> 32) & 0x7FFFFFFFu;
+                    if (qm && !(qm >> 63)) {
+                        rec.mode = OM_NONE; rec.value = 0;                       // "" is falsy
+                        if (tl > 2u) { rec.has = 1; rec.mode = OM_COPY; rec.src_off = ts; rec.src_len = tl; rec.out_len = tl; }
+                    }
+                    uint32_t rdirty = __ballot_sync(0xffffffffu, (qm >> 63) != 0ull);
+                    while (rdirty) {
+                        const int kt = __ffs(rdirty) - 1;
+                        rdirty &= rdirty - 1u;
+                        const uint32_t s0 = __shfl_sync(0xffffffffu, ts, kt), l0 = __shfl_sync(0xffffffffu, tl, kt);
+                        const bool canon = esc_verify_canonical(sbuf, W.soff[kt] + s0 + 1u, l0 - 2u, lane, (uint16_t*)W.ct.ent);
+                        if (canon && lane == kt) { rec.has = 1; rec.mode = OM_COPY; rec.src_off = ts; rec.src_len = tl; rec.out_len = tl; rec.value = 0; }
+                    }
+                }
             }
         } else if (HANDLER == 1) {
             // crc32: the whole warp works on one task at a time (tasks are long and of very different lengths)
             for (uint32_t kt = 0; kt < nt; ++kt) {
                 if (!((ready_mask_t >> kt) & 1u)) continue;
-                if (W.flg[kt] & B9_TF_PICKLE_BIT) { if (lane == (int)kt) rec.status = ST_UNSUPPORTED; continue; }   // function path: identity only
-                if (W.flg[kt] & B9_TF_HTTP_BODY_BIT) {                      // an HTTP body: the sequential parser with the map rules
-                    if (lane == (int)kt) d2_parse_and_size<1>(staged ? (const uint8_t*)(sbuf + W.soff[kt]) : a.payload + W.goff[kt], W.len[kt], rec, s_crc_table, true);
+                const uint32_t fl = W.flg[kt];
+                if (fl & (B9_TF_PICKLE_BIT | B9_TF_HTTP_BODY_BIT | B9_TF_TASK_MSG_BIT)) {
+                    // the function path (identity only), HTTP bodies (map rules), TaskMessage records: the sequential parser
+                    if (lane == (int)kt) {
+                        if (fl & B9_TF_PICKLE_BIT) rec.status = ST_UNSUPPORTED;
+                        else d2_parse_and_size<1>(staged ? (const uint8_t*)(sbuf + W.soff[kt]) : a.payload + W.goff[kt], W.len[kt], rec, s_crc_table,
+                                                   (fl & B9_TF_HTTP_BODY_BIT) != 0,
+                                                   (fl & B9_TF_TASK_MSG_BIT) ? a.ids + ((a.first_task + t0 + kt) & a.slot_mask) : nullptr);
+                    }
                     continue;
                 }
                 const uint8_t* tp = staged ? (const uint8_t*)(sbuf + W.soff[kt]) : stage_one_task(a.payload, W.goff[kt], W.len[kt], sbuf, in_cap, lane);
@@ -1487,9 +1609,15 @@ __global__ void __launch_bounds__(D3_WARPS * 32, (HANDLER == 1 ? B9_CRC_MINB : H
             // json_sum: the whole warp parses one document at a time
             for (uint32_t kt = 0; kt < nt; ++kt) {
                 if (!((ready_mask_t >> kt) & 1u)) continue;
-                if (W.flg[kt] & B9_TF_PICKLE_BIT) { if (lane == (int)kt) rec.status = ST_UNSUPPORTED; continue; }
-                if (W.flg[kt] & B9_TF_HTTP_BODY_BIT) {
-                    if (lane == (int)kt) d2_parse_and_size<3>(staged ? (const uint8_t*)(sbuf + W.soff[kt]) : a.payload + W.goff[kt], W.len[kt], rec, nullptr, true);
+                const uint32_t fl = W.flg[kt];
+                if (fl & (B9_TF_PICKLE_BIT | B9_TF_HTTP_BODY_BIT | B9_TF_TASK_MSG_BIT)) {
+                    // the function path (identity only), HTTP bodies (map rules), TaskMessage records: the sequential parser
+                    if (lane == (int)kt) {
+                        if (fl & B9_TF_PICKLE_BIT) rec.status = ST_UNSUPPORTED;
+                        else d2_parse_and_size<3>(staged ? (const uint8_t*)(sbuf + W.soff[kt]) : a.payload + W.goff[kt], W.len[kt], rec, nullptr,
+                                                   (fl & B9_TF_HTTP_BODY_BIT) != 0,
+                                                   (fl & B9_TF_TASK_MSG_BIT) ? a.ids + ((a.first_task + t0 + kt) & a.slot_mask) : nullptr);
+                    }
                     continue;
                 }
                 int done = 0; unsigned long long sum = 0;
@@ -1507,11 +1635,13 @@ __global__ void __launch_bounds__(D3_WARPS * 32, (HANDLER == 1 ? B9_CRC_MINB : H
             rec.status = ST_UNSUPPORTED;                                   // function path: identity only
         } else if (mine) {
             int fr = 0;
-            if (HANDLER == 2 && staged && !my_http) fr = vadd_fast(sbuf + my_soff, my_len, s_b64, rec);
+            const bool my_rec = (W.flg[k] & B9_TF_TASK_MSG_BIT) != 0;
+            if (HANDLER == 2 && staged && !my_http && !my_rec) fr = vadd_fast(sbuf + my_soff, my_len, s_b64, rec);
             if (fr != 1) {
                 clobbered = fr == 2;                                       // stage bytes overwritten: read the ring instead
                 const uint8_t* p = (staged && !clobbered) ? (const uint8_t*)(sbuf + my_soff) : a.payload + my_goff;
-                d2_parse_and_size<HANDLER>(p, my_len, rec, s_crc_table, my_http);
+                if (my_rec) d2_parse_and_size<HANDLER>(p, my_len, rec, s_crc_table, my_http, a.ids + ((a.first_task + t0 + k) & a.slot_mask));
+                else        d2_parse_and_size<HANDLER>(p, my_len, rec, s_crc_table, my_http);
             }
         }
 
@@ -1549,7 +1679,8 @@ __global__ void __launch_bounds__(D3_WARPS * 32, (HANDLER == 1 ? B9_CRC_MINB : H
                 a.out_ids[j] = (G == 1) ? m_id : __ldg(a.ids + slot);
                 if (HANDLER == 0 && rec.mode == OM_DEFER) {                // the second kernel writes the rest of the record
                     SlowItem* it = a.slow + atomicAdd(&a.ctl->n_slow, 1u);
-                    it->w1 = (unsigned long long)(my_len | (rec.value == 1 ? 0x80000000u : 0u) | (my_http ? 0x40000000u : 0u)) | ((unsigned long long)j << 32) | (rec.value == 2 ? (1ull << 56) : 0ull);
+                    it->w1 = (unsigned long long)(my_len | (rec.value == 1 ? 0x80000000u : 0u) | (my_http ? 0x40000000u : 0u)) | ((unsigned long long)j << 32) | (rec.value == 2 ? (1ull << 56) : 0ull)
+                           | (rec.value == 3 ? (1ull << 57) : 0ull);
                     __threadfence();
                     *(volatile unsigned long long*)&it->w0 = my_goff | ((unsigned long long)a.epoch << 40);
                 } else { a.out_off[j] = fits ? ob : 0; a.out_len[j] = rec.out_len; a.out_status[j] = rec.status; a.out_has[j] = rec.has; }

@@ -20,6 +20,7 @@ __host__ __device__ __forceinline__ uint32_t hdr_len(uint64_t h) { return (uint3
 __host__ __device__ __forceinline__ uint32_t hdr_flags(uint64_t h) { return (uint32_t)(h >> 32) & 0xFFu; }
 constexpr uint32_t B9_TF_HTTP_BODY_BIT = 0x02u;      // == B9_TF_HTTP_BODY (include/b9gpu.h)
 constexpr uint32_t B9_TF_PICKLE_BIT    = 0x04u;      // == B9_TF_PICKLE
+constexpr uint32_t B9_TF_TASK_MSG_BIT  = 0x08u;      // == B9_TF_TASK_MSG
 
 struct DrainCtl {
     unsigned long long ticket;      // next tile to hand out
@@ -37,6 +38,7 @@ struct DrainCtl {
 struct SlowItem {
     unsigned long long w0;          // payload ring offset (40 bits) | epoch << 40
     unsigned long long w1;          // len (30 bits) | bit 30 = HTTP body, bit 31 = the SDK's canonical frame is present | record index (24 bits) << 32 | bit 56 = cloudpickle-framed
+                                    // | bit 57 = a TaskMessage record (B9_TF_TASK_MSG)
 };
 
 struct DrainArgs {

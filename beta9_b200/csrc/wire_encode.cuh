@@ -186,6 +186,7 @@ __global__ void __launch_bounds__(128) wire_encode_kernel(WireArgs a, const Wire
         pr = parse_payload(p, hdr_len(h));
         status = pr.status;
         if (hdr_flags(h) & B9_TF_HTTP_BODY_BIT) status = ST_UNSUPPORTED;     // an HTTP body's TaskPayload follows the map rules: not encoded here
+        if (hdr_flags(h) & B9_TF_TASK_MSG_BIT) status = ST_UNSUPPORTED;      // already a record: nothing to encode
         if (status == ST_OK) {
             if (pr.kw_merged) status = ST_UNSUPPORTED;                       // Go merges duplicate kwargs maps
             if (pr.args_len) la = go_transcode(p, pr.args_off, pr.args_off + pr.args_len, nullptr);

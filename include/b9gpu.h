@@ -103,6 +103,20 @@ enum b9_status {
                                   `str` argument (< 64 KiB of UTF-8), no keyword arguments, handler identity — and reports every
                                   other pickle B9_ST_UNSUPPORTED for the host's CPU loop.                                      */
 
+#define B9_TF_TASK_MSG  0x08u  /* the payload is a TaskMessage record as TaskQueuePop returns it (pkg/abstractions/taskqueue/taskqueue.go:
+                                  238-309): the JSON TaskMessage.Encode writes (pkg/types/task.go:79-90) — a popped record, or the one
+                                  Dispatcher.RetryTask re-encodes (pkg/task/dispatch.go:232-285). The drain runs the runner's half of the
+                                  loop on it: json.loads, the handler, serialize_result (sdk/src/beta9/runner/taskqueue.py:196-201,349-378).
+                                  Results and statuses go into b9_results like any other task's; the record id is the slot's id from the
+                                  push, which must be the record's "task_id". B9_ST_REJECTED never comes out of this path (the task exists).
+                                  The device answers a record only where CPython's reading of it equals its reading of Go's re-encoding
+                                  (DESIGN.md §4 "Queue records"): the whole record UTF-8, strict JSON, "task_id" / "args" / "kwargs" once
+                                  each and exact, args a list or null, kwargs an object or null; inside them no lone or encoded surrogate,
+                                  every number exactly Go's float text, object keys sorted and unique. Every record TaskMessage.Encode
+                                  writes is inside; anything else is B9_ST_UNSUPPORTED, and so is TASK_MSG together with HTTP_BODY or
+                                  PICKLE. b9_wire_encode reports a TASK_MSG task UNSUPPORTED. The host fills b9_push_meta's timestamp /
+                                  expires / retries from the record it decoded; the device does not read them from the bytes.        */
+
 typedef struct b9_ctx b9_ctx;
 
 typedef struct b9_opts {
