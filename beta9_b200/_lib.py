@@ -13,6 +13,7 @@ H_IDENTITY, H_CRC32, H_VADD_F32, H_JSON_SUM = 0, 1, 2, 3
 ST_COMPLETE, ST_ERROR, ST_RETRY, ST_REJECTED, ST_UNSUPPORTED = 0, 1, 2, 3, 4
 TF_CANCELLED = 0x01
 TF_HTTP_BODY, TF_PICKLE, TF_TASK_MSG = 0x02, 0x04, 0x08
+CANCEL_MARKED, CANCEL_ALREADY, CANCEL_CLAIMED = 0x01, 0x02, 0x04      # b9_cancel outcome bits
 
 
 class Opts(C.Structure):
@@ -78,6 +79,7 @@ SYMBOLS = {
     "b9_running": (C.c_uint64, [C.c_void_p]),
     "b9_depth_bytes": (C.c_uint64, [C.c_void_p]),
     "b9_expire": (C.c_int64, [C.c_void_p, C.c_int64]),
+    "b9_cancel": (C.c_int64, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]),
     "b9_drain": (C.c_int64, [C.c_void_p, C.c_int, C.c_uint32, C.POINTER(Results)]),
     "b9_drain_launch": (C.c_int64, [C.c_void_p, C.c_int, C.c_uint32, C.c_int]),
     "b9_drain_fetch": (C.c_int64, [C.c_void_p, C.POINTER(Results)]),

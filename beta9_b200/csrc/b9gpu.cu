@@ -25,6 +25,7 @@
 #include <vector>
 
 #include "../../include/b9gpu.h"
+#include "cancel.cuh"
 #include "drain_kernel.cuh"
 #include "drain2.cuh"
 #include "rebalance_plan.h"
@@ -111,7 +112,7 @@ struct b9_ctx {
     cudaEvent_t ev_a = nullptr, ev_b = nullptr, ev_c = nullptr, ev_d = nullptr;   // drain stream (under out_mu)
     cudaEvent_t ev_pa = nullptr, ev_pb = nullptr;                                    // ingest stream (under in_mu)
     // Three locks, always taken in this order: in_mu (push submission: H2D + ingest kernel are enqueued in FIFO order),
-    // out_mu (drain-side submission and the waiting-results state: launch, fetch, expire, wire records, rebalance), mu
+    // out_mu (drain-side submission and the waiting-results state: launch, fetch, expire, cancel, wire records, rebalance), mu
     // (ring bookkeeping + stats; held for pointer arithmetic only, never across a CUDA synchronisation). Producers
     // therefore never wait for a drain's kernels or its D2H copy, and the drainer never waits for a push's DMA
     // (Dispatcher.Register's goroutine-safety contract, pkg/task/dispatch.go:71-73).
@@ -144,7 +145,8 @@ struct b9_ctx {
     uint32_t drain_epoch = 0;                   // tag of the current launch's work-list items
     WireEnv* d_wire_env = nullptr;
     uint32_t* d_crc_shift = nullptr;            // crc32: zero-byte shift tables
-    uint64_t cancelled_pending = 0;            // pending tasks carrying B9_TF_CANCELLED (pushed so, or expired)
+    uint64_t cancelled_pending = 0;            // pending tasks carrying B9_TF_CANCELLED (pushed so, expired, or b9_cancel)
+    CancelKey* d_cancel_keys = nullptr; uint32_t* d_cancel_out = nullptr; uint32_t cancel_cap = 0;   // b9_cancel: sorted ids + outcome words, grow-only
     DrainCtl* d_ctl = nullptr; uint64_t* d_tile_state = nullptr;
     bool burst_open = false; cudaEvent_t ev_burst = nullptr;   // B9_DRAIN_ASYNC launches since the last completion: timed as one burst
     bool res_async = false;                    // the last launch returned before its kernels finished: finalize on fetch / sync
@@ -415,6 +417,7 @@ void b9_ctx_destroy(b9_ctx* c) {
     cudaFree(c->d_in_off); cudaFree(c->d_in_ts); cudaFree(c->d_in_exp); cudaFree(c->d_in_retries); cudaFree(c->d_in_flags);
     cudaFree(c->d_out_payload); cudaFree(c->d_out_off); cudaFree(c->d_out_ids); cudaFree(c->d_out_status); cudaFree(c->d_out_has); cudaFree(c->d_out_len); cudaFree(c->d_slow); cudaFree(c->d_wire_env); cudaFree(c->d_crc_shift);
     cudaFree(c->d_ctl); cudaFree(c->d_tile_state); cudaFree(c->d_count);
+    cudaFree(c->d_cancel_keys); cudaFree(c->d_cancel_out);
     if (c->h_ctl) cudaFreeHost(c->h_ctl);
     if (c->h_rtab) cudaFreeHost(c->h_rtab);
     cudaFree(c->d_rtab); cudaFree(c->d_prefix); cudaFree(c->d_scan_sums);
@@ -755,6 +758,60 @@ int64_t b9_expire(b9_ctx* c, int64_t now_unix_ns) {
     c->cancelled_pending += *c->h_count;
     c->expired_since_launch = true;
     return (int64_t)*c->h_count;
+}
+
+// StopTasks (pkg/api/v1/task.go:333-398) for the pending tasks of this ctx: cancel_kernel (cancel.cuh) over the ring.
+// The claimed window of an outstanding drain is looked up but never written, so b9_drain_fetch's
+// `cancelled_pending -= popped - records` stays exact without a recount.
+int64_t b9_cancel(b9_ctx* c, const uint8_t* task_ids, uint32_t n, uint8_t* outcome) {
+    if (!c) return fail(B9_EINVAL, "b9_cancel: ctx is NULL");
+    if (n && !task_ids) return fail(B9_EINVAL, "b9_cancel: task_ids is NULL");
+    if (n > (1u << 20)) return fail(B9_E2BIG, "b9_cancel: %u ids in one call, at most 2^20", n);
+    if (outcome && n) memset(outcome, 0, n);
+    if (n == 0) return 0;
+    // sorted outside the locks: producers and drains do not wait for it
+    std::vector<CancelKey> keys; std::vector<uint32_t> which;
+    try { cancel_sort_unique(task_ids, n, keys, which); } catch (const std::bad_alloc&) { return fail(B9_ENOMEM, "b9_cancel: host allocation failed"); }
+    const uint32_t n_keys = (uint32_t)keys.size();
+    std::lock_guard<std::mutex> out_lk(c->out_mu);
+    CU(cudaSetDevice(c->device));
+    cudaStream_t s = c->stream;
+    uint64_t head = 0, depth = 0;
+    {
+        std::lock_guard<std::mutex> lk(c->mu);
+        head = c->head_task; depth = c->tail_task - c->head_task;
+        if (!depth) return 0;
+        for (const Segment& sg : c->segs) CU(cudaStreamWaitEvent(s, sg.ready, 0));
+    }
+    const uint32_t claimed = (uint32_t)std::min<uint64_t>(c->running.load(std::memory_order_relaxed), depth);   // (set and cleared under out_mu)
+    if (c->cancel_cap < n_keys) {
+        cudaFree(c->d_cancel_keys); cudaFree(c->d_cancel_out);
+        c->d_cancel_keys = nullptr; c->d_cancel_out = nullptr; c->cancel_cap = 0;
+        cudaError_t e = cudaMalloc(&c->d_cancel_keys, (size_t)n_keys * sizeof(CancelKey));
+        if (e == cudaSuccess) e = cudaMalloc(&c->d_cancel_out, (size_t)n_keys * sizeof(uint32_t));
+        if (e != cudaSuccess) { cudaGetLastError(); return fail(e == cudaErrorMemoryAllocation ? B9_ENOMEM : B9_EIO, "b9_cancel: %u keys: %s", n_keys, cudaGetErrorString(e)); }
+        c->cancel_cap = n_keys;
+    }
+    CU(cudaMemcpyAsync(c->d_cancel_keys, keys.data(), (size_t)n_keys * sizeof(CancelKey), cudaMemcpyHostToDevice, s));
+    CU(cudaMemsetAsync(c->d_cancel_out, 0, (size_t)n_keys * sizeof(uint32_t), s));
+    CU(cudaMemsetAsync(c->d_count, 0, sizeof(unsigned long long), s));
+    const uint32_t stride = cancel_fence_stride(n_keys), n_fence = (n_keys + stride - 1u) / stride;
+    const uint32_t grid = (uint32_t)std::min<uint64_t>((depth + 255) / 256, (uint64_t)c->sm_count * 8u);
+    cancel_kernel<<<grid, 256, (size_t)n_fence * sizeof(CancelKey), s>>>(c->d_hdr, c->d_ids, c->slot_mask, head, claimed, (uint32_t)depth,
+                                                                         c->d_cancel_keys, n_keys, stride, n_fence, c->d_cancel_out, c->d_count);
+    CU(cudaGetLastError());
+    std::vector<uint32_t> words(n_keys);
+    CU(cudaMemcpyAsync(words.data(), c->d_cancel_out, (size_t)n_keys * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(c->h_count, c->d_count, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    const uint64_t marked = *c->h_count;
+    {
+        std::lock_guard<std::mutex> lk(c->mu);
+        c->stats.kernel_launches++;
+        c->cancelled_pending += marked;
+    }
+    if (outcome) for (uint32_t i = 0; i < n; ++i) outcome[i] = (uint8_t)words[which[i]];
+    return (int64_t)marked;
 }
 
 // Waits for the last launch and publishes its outcome (records, bytes, overflow) to the ctx. Caller holds c->out_mu (not c->mu).

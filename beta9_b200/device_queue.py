@@ -162,6 +162,15 @@ class DeviceQueue:
     def expire(self, now_unix_ns: int) -> int:    # dispatch.go:173-230 monitor, unclaimed branch
         return self._check(self._lib.b9_expire(self._ctx, now_unix_ns))
 
+    def cancel(self, task_ids: np.ndarray) -> Tuple[int, np.ndarray]:   # api/v1/task.go:333-398 StopTasks
+        """b9_cancel: marks the pending, unclaimed tasks with these ids (uint8 [n,16]) cancelled. Returns (slots marked,
+        uint8 [n] outcome: an OR of CANCEL_MARKED / CANCEL_ALREADY / CANCEL_CLAIMED, 0 = no such pending task)."""
+        ids = np.ascontiguousarray(task_ids, dtype=np.uint8).reshape(-1, 16)
+        n = ids.shape[0]
+        outcome = np.zeros(max(n, 1), np.uint8)
+        marked = self._check(self._lib.b9_cancel(self._ctx, ids.ctypes.data if n else None, n, outcome.ctypes.data))
+        return marked, outcome[:n]
+
     # ---- consumer side
     def drain(self, handler: str, max_tasks: int = 1 << 22, cap_bytes: Optional[int] = None) -> DrainResult:
         h = HANDLERS[handler]

@@ -16,14 +16,16 @@ import json
 import os
 import uuid
 from dataclasses import dataclass
-from typing import Any, Callable, Iterator, List, Optional, Sequence, Union
+from typing import Any, Callable, Dict, Iterator, List, Optional, Sequence, Union
 
 import numpy as np
 
+from . import _lib as L
 from .device_queue import DeviceQueue, STATUS_NAMES
 
 TASKQUEUE_STUB_TYPE = "taskqueue"
 DEFAULT_MAX_PENDING_TASKS = 100      # sdk/src/beta9/abstractions/taskqueue.py:142
+_CANCEL_MAX_IDS = 1 << 20            # most ids one b9_cancel takes
 
 
 @dataclass
@@ -147,6 +149,27 @@ class _CallableWrapper:
         if isinstance(c, list):
             return tuple(c), {}
         return (c,), {}
+
+    def stop_tasks(self, task_ids: Sequence[str]) -> Dict[str, str]:
+        """The gateway's StopTasks (pkg/api/v1/task.go:333-398) for this queue: every pending task with one of these ids is
+        cancelled and produces no record. Per id: "CANCELLED", "ALREADY_CANCELLED", "RUNNING" (claimed by a drain in flight:
+        left alone) or "NOT_FOUND"; ids that are unknown or not UUIDs are ignored, as the reference ignores them."""
+        names = {str(t): "NOT_FOUND" for t in task_ids}
+        raw = []
+        for t in names:
+            try:
+                raw.append((t, uuid.UUID(t).bytes))
+            except ValueError:
+                continue
+        q = self.parent.queue
+        for lo in range(0, len(raw), _CANCEL_MAX_IDS):
+            part = raw[lo:lo + _CANCEL_MAX_IDS]
+            ids = np.frombuffer(b"".join(b for _, b in part), np.uint8).reshape(-1, 16)
+            _, outcome = q.cancel(ids)
+            for (t, _), o in zip(part, outcome):
+                names[t] = ("CANCELLED" if o & L.CANCEL_MARKED else "ALREADY_CANCELLED" if o & L.CANCEL_ALREADY
+                            else "RUNNING" if o & L.CANCEL_CLAIMED else "NOT_FOUND")
+        return names
 
     # ---- consumer (what the runner loop + TaskQueueComplete hand back)
     def process_tasks(self, max_tasks: int = 1 << 22) -> List[Task]:

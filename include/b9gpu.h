@@ -20,7 +20,7 @@
  *   - thread safety: all functions may be called concurrently from many OS threads (goroutine
  *     backed or not). Producers and the drainer of one ctx run CONCURRENTLY: pushes serialise among
  *     themselves (FIFO order is the order in which they are enqueued), drain-side calls (launch,
- *     fetch, expire, wire records) serialise among themselves, and neither side waits for the
+ *     fetch, expire, cancel, wire records) serialise among themselves, and neither side waits for the
  *     other's DMA or kernels. b9_rebalance excludes both for its duration.
  *   - a batch is packed SoA: `task_ids` n x 16 raw UUID bytes, `payload` one blob, `offsets`
  *     n+1 byte offsets into it. A task's payload is the exact `TaskQueuePutRequest.payload`
@@ -246,6 +246,24 @@ uint64_t b9_running(b9_ctx *ctx);
 /* Marks every pending task whose expires_unix_ns is non-zero and <= now as cancelled — the
  * unclaimed-task branch of `Dispatcher.monitor` (pkg/task/dispatch.go:173-230). Returns count. */
 int64_t  b9_expire(b9_ctx *ctx, int64_t now_unix_ns);
+
+/* Cancels pending tasks by id — `StopTasks` (pkg/api/v1/task.go:333-398), which marks a task cancelled so that
+ * TaskQueuePop skips it (taskqueue.go:238-270). Every pending, unclaimed slot whose 16-byte id equals one of the n
+ * `task_ids` (n x 16 raw UUID bytes) gets B9_TF_CANCELLED, duplicates of one id included (the reference keys state by
+ * id); the drain then compacts it away like a task pushed so. Covers every task whose push returned before the call;
+ * tasks still in the submission arena (b9_buffered) are not pending yet: b9_flush first. The claimed window of an
+ * outstanding drain (b9_running) is never touched: its records come back with that drain's b9_drain_fetch, as a task
+ * a runner has already popped. After a B9_DRAIN_PEEK launch nothing is claimed. A drain-side call.
+ * `outcome` (NULL or [n]): per requested id, an OR of the bits below (0 = no pending task with this id on this ctx);
+ * the copies of one id in the list get the same byte. Returns the number of slots marked, or B9_EINVAL (NULL ctx,
+ * NULL ids with n > 0), B9_E2BIG (n > 2^20: split the list), B9_ENOMEM, B9_EIO. b9_depth / b9_depth_bytes count a
+ * cancelled task until a drain pops it. Added without an ABI version change: probe for it with dlsym. */
+#define B9_CANCEL_MARKED   0x01u  /* at least one pending, unclaimed task with this id was cancelled by this call       */
+#define B9_CANCEL_ALREADY  0x02u  /* a pending task with this id already carried B9_TF_CANCELLED (pushed so, expired,
+                                     cancelled)                                                                        */
+#define B9_CANCEL_CLAIMED  0x04u  /* a task with this id is in the window of an outstanding drain: left alone, its record
+                                     comes back with that drain's b9_drain_fetch                                        */
+int64_t  b9_cancel(b9_ctx *ctx, const uint8_t *task_ids, uint32_t n, uint8_t *outcome);
 
 /* ---- consumer side ---------------------------------------------------------------------------
  * b9_drain replaces, for up to max_tasks pending tasks in FIFO order, the whole
