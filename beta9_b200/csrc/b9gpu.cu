@@ -61,6 +61,7 @@ struct Segment {             // one push = one contiguous byte range of the payl
     uint64_t phys_start, bytes;
     cudaEvent_t ready;           // recorded on the ingest stream once the batch is fully on the device
     uint32_t max_len = 0;        // longest task of the batch (0 = not known: tasks that arrived in a rebalance)
+    bool drain_waited = false;   // a drain launch has made the drain stream wait for `ready` (stream order covers later launches)
 };
 
 constexpr uint64_t RING_SLACK = 256;   // readable bytes past the ring end (vector loads may over-read)
@@ -147,8 +148,13 @@ struct b9_ctx {
     uint32_t* d_crc_shift = nullptr;            // crc32: zero-byte shift tables
     uint64_t cancelled_pending = 0;            // pending tasks carrying B9_TF_CANCELLED (pushed so, expired, or b9_cancel)
     CancelKey* d_cancel_keys = nullptr; uint32_t* d_cancel_out = nullptr; uint32_t cancel_cap = 0;   // b9_cancel: sorted ids + outcome words, grow-only
-    DrainCtl* d_ctl = nullptr; uint64_t* d_tile_state = nullptr;
-    bool burst_open = false; cudaEvent_t ev_burst = nullptr;   // B9_DRAIN_ASYNC launches since the last completion: timed as one burst
+    DrainCtl* d_ctl = nullptr; uint64_t* d_tile_state = nullptr;   // d_ctl: D3_CTL_RING control blocks (drain_kernel.cuh)
+    bool ctl_dirty = false;                    // the next drain's control block may be non-zero: zero the ring before it
+    uint32_t ctl_last = 0;                     // control block of the last drain launch (read by finish_launch)
+    bool last_op_drain = false;                // the drain stream's last operation is a drain3_kernel: the next may overlap it
+    // launches since the last completion are timed as one span: ev_burst before the first one's kernel, ev_b right after
+    // the last one's (recorded before anything else is enqueued on the drain stream, see end_drain_span)
+    bool burst_open = false; cudaEvent_t ev_burst = nullptr;
     bool res_async = false;                    // the last launch returned before its kernels finished: finalize on fetch / sync
     uint32_t res_async_n = 0; uint64_t res_async_in_bytes = 0;
     DrainCtl* h_ctl = nullptr;                 // pinned
@@ -177,12 +183,28 @@ void free_segments(b9_ctx* c) {
     if (c->segs.empty()) c->write_pos = 0;
 }
 
+// Closes the timed span of the drain launches enqueued so far (ev_b right behind the last drain kernel), before anything
+// else goes on the drain stream. Caller holds c->out_mu.
+void end_drain_span(b9_ctx* c) {
+    if (!c->last_op_drain) return;
+    c->last_op_drain = false;
+    cudaSetDevice(c->device);
+    cudaEventRecord(c->ev_b, c->stream);
+}
+
+// c->out_mu for every drain-stream user except b9_drain_launch: whatever it enqueues comes after the open span's end
+struct OutLock {
+    std::lock_guard<std::mutex> lk;
+    explicit OutLock(b9_ctx* c) : lk(c->out_mu) { end_drain_span(c); }
+};
+
 // Physical payload offset of logical task `idx` of segment `sg` (idx == first_task + n gives the segment's
 // end). Only partial-segment operations need it (a drain that stops inside a batch, the rebalance), so
 // the host keeps no per-task index: the slot ring on the device is the index. Synchronous, 8 bytes.
 int task_phys_off(b9_ctx* c, const Segment& sg, uint64_t idx, uint64_t* out) {
     if (idx == sg.first_task) { *out = sg.phys_start; return B9_OK; }
     if (idx == sg.first_task + sg.n) { *out = sg.phys_start + sg.bytes; return B9_OK; }
+    c->last_op_drain = false;
     CU(cudaStreamWaitEvent(c->stream, sg.ready, 0));
     CU(cudaMemcpyAsync(&c->h_ctl->total, c->d_off + (uint32_t)(idx & c->slot_mask), sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
@@ -202,7 +224,10 @@ template <int H> uint32_t drain3_warp_stride(uint32_t in_cap) {
     const size_t ctl = (sizeof(D3Warp<D3Cfg<H>::T>) + 127u) & ~(size_t)127u;
     return (uint32_t)(ctl + (((size_t)in_cap + 64u + 127u) & ~(size_t)127u));
 }
-template <int H> cudaError_t launch_drain3(DrainArgs a, uint64_t avg_task_bytes, uint32_t max_task_len, uint32_t cap_override, int sm_count, cudaStream_t s, int* grid_out) {
+// overlap: the drain stream's last operation is a drain3_kernel and the window has no cancelled slot (so no count kernels
+// run first): the kernel is launched as that one's programmatic dependent — its CTAs become resident as the previous
+// grid's leave, and it waits for that grid's completion (griddepcontrol.wait) before it touches anything a drain writes
+template <int H> cudaError_t launch_drain3(DrainArgs a, uint64_t avg_task_bytes, uint32_t max_task_len, uint32_t cap_override, int sm_count, bool overlap, cudaStream_t s, int* grid_out) {
     constexpr int T = D3Cfg<H>::T;
     static const bool tight = !(getenv("B9_STAGE_TIGHT") && atoi(getenv("B9_STAGE_TIGHT")) == 0);      // (=0: the A/B switch)
     uint32_t in_cap = 0, stride = 0; size_t smem = 0; int per_sm = 0;
@@ -264,7 +289,15 @@ template <int H> cudaError_t launch_drain3(DrainArgs a, uint64_t avg_task_bytes,
         const uint64_t rounds = a.n_tiles / ((uint64_t)grid * D3_WARPS);
         a.static_rounds = rounds > dyn ? (uint32_t)(rounds - dyn) : 0u;
     }
-    drain3_kernel<H><<<grid, D3_WARPS * 32, smem, s>>>(a, in_cap, stride);
+    a.static_rounds = std::max(a.static_rounds, 1u);                       // every worker's first tile is static (drain3_kernel)
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3(D3_WARPS * 32); cfg.dynamicSmemBytes = smem; cfg.stream = s;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr; cfg.numAttrs = (overlap && !a.count_mode) ? 1 : 0;
+    e = cudaLaunchKernelEx(&cfg, drain3_kernel<H>, a, in_cap, stride);
+    if (e != cudaSuccess) return e;
     return cudaGetLastError();
 }
 
@@ -393,7 +426,8 @@ int b9_ctx_create(const b9_opts* opts, b9_ctx** out) {
         CUC(cudaMalloc(&c->d_crc_shift, tabs.size() * sizeof(uint32_t)));
         CUC(cudaMemcpy(c->d_crc_shift, tabs.data(), tabs.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
     }
-    CUC(cudaMalloc(&c->d_ctl, sizeof(DrainCtl)));
+    CUC(cudaMalloc(&c->d_ctl, D3_CTL_RING * sizeof(DrainCtl)));
+    CUC(cudaMemset(c->d_ctl, 0, D3_CTL_RING * sizeof(DrainCtl)));
     CUC(cudaMalloc(&c->d_tile_state, ((size_t)md / D2_THREADS + 2) * sizeof(uint64_t)));
     CUC(cudaMalloc(&c->d_count, sizeof(unsigned long long)));
     CUC(cudaHostAlloc(&c->h_ctl, sizeof(DrainCtl), cudaHostAllocDefault));
@@ -739,7 +773,7 @@ uint64_t b9_running(b9_ctx* c) { return c ? c->running.load(std::memory_order_re
 
 int64_t b9_expire(b9_ctx* c, int64_t now_unix_ns) {
     if (!c) return fail(B9_EINVAL, "b9_expire: ctx is NULL");
-    std::lock_guard<std::mutex> out_lk(c->out_mu);
+    OutLock out_lk(c);
     CU(cudaSetDevice(c->device));
     uint64_t head = 0, depth = 0;
     {
@@ -773,7 +807,7 @@ int64_t b9_cancel(b9_ctx* c, const uint8_t* task_ids, uint32_t n, uint8_t* outco
     std::vector<CancelKey> keys; std::vector<uint32_t> which;
     try { cancel_sort_unique(task_ids, n, keys, which); } catch (const std::bad_alloc&) { return fail(B9_ENOMEM, "b9_cancel: host allocation failed"); }
     const uint32_t n_keys = (uint32_t)keys.size();
-    std::lock_guard<std::mutex> out_lk(c->out_mu);
+    OutLock out_lk(c);
     CU(cudaSetDevice(c->device));
     cudaStream_t s = c->stream;
     uint64_t head = 0, depth = 0;
@@ -818,10 +852,11 @@ int64_t b9_cancel(b9_ctx* c, const uint8_t* task_ids, uint32_t n, uint8_t* outco
 static int finish_launch(b9_ctx* c) {
     if (!c->res_async) return B9_OK;
     c->res_async = false;
-    CU(cudaMemcpyAsync(c->h_ctl, c->d_ctl, sizeof(DrainCtl), cudaMemcpyDeviceToHost, c->stream));
+    end_drain_span(c);
+    CU(cudaMemcpyAsync(c->h_ctl, c->d_ctl + c->ctl_last, sizeof(DrainCtl), cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
     // one launch: the time around its kernels; a burst of B9_DRAIN_ASYNC launches: from the first one's start to the last one's end
-    float ms = 0; cudaEventElapsedTime(&ms, c->burst_open ? c->ev_burst : c->ev_a, c->ev_b);
+    float ms = 0; cudaEventElapsedTime(&ms, c->ev_burst, c->ev_b);
     c->burst_open = false;
     c->res_kernel_ms = ms;
     if (c->h_ctl->overflow) {
@@ -853,7 +888,7 @@ int64_t b9_drain_launch(b9_ctx* c, int handler, uint32_t max_tasks, int peek) {
     cudaStream_t s = c->stream;
     // the window: a snapshot of the ring's head under the bookkeeping lock. Only drain-side calls (all under out_mu)
     // move the head or free segments, so the snapshot stays valid while the launch is prepared without c->mu.
-    struct Piece { Segment sg; uint64_t a, b; };
+    struct Piece { Segment sg; uint64_t a, b; bool wait; };
     std::vector<Piece> pieces;
     uint64_t head = 0; uint32_t n = 0; uint32_t count_mode = 0;
     {
@@ -864,9 +899,9 @@ int64_t b9_drain_launch(b9_ctx* c, int handler, uint32_t max_tasks, int peek) {
         count_mode = c->cancelled_pending ? 1u : 0u;
         c->expired_since_launch = false;
         const uint64_t lo = head, hi = head + n;
-        for (const Segment& sg : c->segs) {
+        for (Segment& sg : c->segs) {
             const uint64_t a = std::max<uint64_t>(lo, sg.first_task), b = std::min<uint64_t>(hi, sg.first_task + sg.n);
-            if (a < b) pieces.push_back(Piece{sg, a, b});
+            if (a < b) { pieces.push_back(Piece{sg, a, b, !sg.drain_waited}); sg.drain_waited = true; }
         }
     }
     if (n == 0) { c->have_results = true; return 0; }
@@ -875,7 +910,10 @@ int64_t b9_drain_launch(b9_ctx* c, int handler, uint32_t max_tasks, int peek) {
     for (const Piece& pc : pieces) { if (pc.sg.max_len) win_max_len = std::max(win_max_len, pc.sg.max_len); else max_known = false; }
     if (!max_known) win_max_len = 0;
     for (const Piece& pc : pieces) {
-        CU(cudaStreamWaitEvent(s, pc.sg.ready, 0));                         // this batch's H2D + ingest must have landed
+        if (pc.wait) {                                                      // this batch's H2D + ingest must have landed
+            c->last_op_drain = false;                                       // (once per segment: stream order covers later drains)
+            CU(cudaStreamWaitEvent(s, pc.sg.ready, 0));
+        }
         uint64_t o0 = 0, o1 = 0;
         int rc = task_phys_off(c, pc.sg, pc.a, &o0); if (rc) return rc;
         rc = task_phys_off(c, pc.sg, pc.b, &o1); if (rc) return rc;
@@ -885,28 +923,42 @@ int64_t b9_drain_launch(b9_ctx* c, int handler, uint32_t max_tasks, int peek) {
     a.payload = c->d_payload; a.off = c->d_off; a.hdr = c->d_hdr; a.ids = c->d_ids; a.slot_mask = c->slot_mask;
     a.first_task = head; a.n_tasks = n; a.n_tiles = 0;                     // (set per handler by launch_drain3)
     a.out_payload = c->d_out_payload; a.out_cap = c->max_result_bytes; a.out_off = c->d_out_off; a.out_ids = c->d_out_ids;
-    a.out_status = c->d_out_status; a.out_has = c->d_out_has; a.out_len = c->d_out_len; a.ctl = c->d_ctl; a.tile_base = (const uint32_t*)c->d_tile_state; a.block_base = (const uint32_t*)c->d_tile_state + ((size_t)c->max_drain_tasks / D2_THREADS + 2); a.handler = handler;
+    a.out_status = c->d_out_status; a.out_has = c->d_out_has; a.out_len = c->d_out_len; a.tile_base = (const uint32_t*)c->d_tile_state; a.block_base = (const uint32_t*)c->d_tile_state + ((size_t)c->max_drain_tasks / D2_THREADS + 2); a.handler = handler;
     a.count_mode = count_mode;
     a.slow = c->d_slow; a.crc_shift_tabs = c->d_crc_shift;
     a.static_rounds = 0;
     c->drain_epoch = (c->drain_epoch + 1u) & 0xFFFFFFu;
-    if (c->drain_epoch == 0u) { c->drain_epoch = 1u; CU(cudaMemsetAsync(c->d_slow, 0, (size_t)c->max_drain_tasks * sizeof(SlowItem), s)); }   // the 24-bit tag wrapped: forget old tags
+    if (c->drain_epoch == 0u) {                                             // the 24-bit tag wrapped: forget old tags
+        c->drain_epoch = 1u; c->ctl_dirty = true;                           // (and the control ring's order)
+        c->last_op_drain = false;
+        CU(cudaMemsetAsync(c->d_slow, 0, (size_t)c->max_drain_tasks * sizeof(SlowItem), s));
+    }
     a.epoch = c->drain_epoch;
-    CU(cudaMemsetAsync(c->d_ctl, 0, sizeof(DrainCtl), s));
+    // the control block: the previous drain kernel zeroed this one (drain_kernel.cuh, D3_CTL_RING), unless something
+    // else ran since that the host cannot see through (a failed launch, the wire encoder, the epoch's wrap)
+    c->ctl_last = a.epoch % D3_CTL_RING;
+    a.ctl = c->d_ctl + c->ctl_last; a.ctl_next = c->d_ctl + (a.epoch + 1u) % D3_CTL_RING;
+    if (c->ctl_dirty) {
+        c->last_op_drain = false;
+        CU(cudaMemsetAsync(c->d_ctl, 0, D3_CTL_RING * sizeof(DrainCtl), s));
+        c->ctl_dirty = false;
+    }
     int grid = 0;
-    if (!c->burst_open) CU(cudaEventRecord(c->ev_burst, s));
-    CU(cudaEventRecord(c->ev_a, s));
+    if (!c->burst_open) { c->last_op_drain = false; CU(cudaEventRecord(c->ev_burst, s)); }
+    // within a burst nothing is enqueued between one launch's kernel and the next one's: the span's end event is recorded
+    // by whatever comes next (end_drain_span), the control block is read back by finish_launch
+    const bool overlap = c->last_op_drain;
+    c->last_op_drain = false;
     cudaError_t le;
     switch (handler) {
-    case B9_H_IDENTITY: le = launch_drain3<0>(a, in_bytes / n, win_max_len, c->stage_bytes_override, c->sm_count, s, &grid); break;
-    case B9_H_CRC32:    le = launch_drain3<1>(a, in_bytes / n, win_max_len, c->stage_bytes_override, c->sm_count, s, &grid); break;
-    case B9_H_VADD_F32: le = launch_drain3<2>(a, in_bytes / n, win_max_len, c->stage_bytes_override, c->sm_count, s, &grid); break;
-    default:            le = launch_drain3<3>(a, in_bytes / n, win_max_len, c->stage_bytes_override, c->sm_count, s, &grid); break;
+    case B9_H_IDENTITY: le = launch_drain3<0>(a, in_bytes / n, win_max_len, c->stage_bytes_override, c->sm_count, overlap, s, &grid); break;
+    case B9_H_CRC32:    le = launch_drain3<1>(a, in_bytes / n, win_max_len, c->stage_bytes_override, c->sm_count, overlap, s, &grid); break;
+    case B9_H_VADD_F32: le = launch_drain3<2>(a, in_bytes / n, win_max_len, c->stage_bytes_override, c->sm_count, overlap, s, &grid); break;
+    default:            le = launch_drain3<3>(a, in_bytes / n, win_max_len, c->stage_bytes_override, c->sm_count, overlap, s, &grid); break;
     }
-    if (le != cudaSuccess) return fail(B9_EIO, "drain kernel launch failed: %s", cudaGetErrorString(le));
-    CU(cudaEventRecord(c->ev_b, s));
-    // (the control block is read back by finish_launch: a burst of B9_DRAIN_ASYNC launches then has no copy-engine
-    // operation between one launch's kernel and the next one's)
+    if (le != cudaSuccess) { c->ctl_dirty = true; return fail(B9_EIO, "drain kernel launch failed: %s", cudaGetErrorString(le)); }
+    c->last_op_drain = true;
+    c->burst_open = true;
     {
         std::lock_guard<std::mutex> lk(c->mu);
         c->stats.kernel_launches += a.count_mode ? 3 : 1;                  // (+ tile_count_kernel and tile_scan_kernel)
@@ -915,14 +967,14 @@ int64_t b9_drain_launch(b9_ctx* c, int handler, uint32_t max_tasks, int peek) {
     }
     c->res_async = true; c->res_async_n = n; c->res_async_in_bytes = in_bytes;
     if (!c->res_peek) c->running.store(n, std::memory_order_relaxed);
-    if (peek & B9_DRAIN_ASYNC) { c->burst_open = true; return (int64_t)n; }   // records = n minus the cancelled slots: known after b9_sync / b9_drain_fetch
+    if (peek & B9_DRAIN_ASYNC) return (int64_t)n;   // records = n minus the cancelled slots: known after b9_sync / b9_drain_fetch
     int rc = finish_launch(c);
     return rc ? rc : (int64_t)c->res_n;
 }
 
 int64_t b9_drain_fetch(b9_ctx* c, b9_results* out) {
     if (!c || !out) return fail(B9_EINVAL, "b9_drain_fetch: NULL argument");
-    std::lock_guard<std::mutex> out_lk(c->out_mu);
+    OutLock out_lk(c);
     CU(cudaSetDevice(c->device));
     { int rc = finish_launch(c); if (rc) return rc; }
     if (!c->have_results) return fail(B9_EINVAL, "b9_drain_fetch: no drain results are waiting");
@@ -1007,7 +1059,7 @@ static size_t host_go_quote(const char* s, uint8_t* o, size_t cap) {
 
 int64_t b9_wire_encode(b9_ctx* c, const b9_wire_env* env, uint32_t max_tasks) {
     if (!c || !env || !env->workspace_name || !env->stub_id) return fail(B9_EINVAL, "b9_wire_encode: NULL argument");
-    std::lock_guard<std::mutex> out_lk(c->out_mu);
+    OutLock out_lk(c);
     CU(cudaSetDevice(c->device));
     c->have_results = false; c->res_async = false; c->burst_open = false;
     c->running.store(0, std::memory_order_relaxed);
@@ -1035,7 +1087,8 @@ int64_t b9_wire_encode(b9_ctx* c, const b9_wire_env* env, uint32_t max_tasks) {
     }
     we.max_retries = env->max_retries; we.timeout = env->timeout; we.ttl = env->ttl;
     CU(cudaMemcpyAsync(c->d_wire_env, &we, sizeof we, cudaMemcpyHostToDevice, s));
-    CU(cudaMemsetAsync(c->d_ctl, 0, sizeof(DrainCtl), s));
+    CU(cudaMemsetAsync(c->d_ctl, 0, sizeof(DrainCtl), s));                  // (the control ring's first entry: the next drain zeroes the ring)
+    c->ctl_dirty = true;
     WireArgs a{};
     a.payload = c->d_payload; a.off = c->d_off; a.hdr = c->d_hdr; a.ids = c->d_ids; a.ts = c->d_ts; a.exp = c->d_exp;
     a.slot_mask = c->slot_mask; a.first_task = head; a.n_tasks = n;
@@ -1281,7 +1334,7 @@ int b9_comm_init(b9_ctx* c, const uint8_t* id128, int rank, int world) {
     if (world > REBALANCE_MAX_WORLD) return fail(B9_EINVAL, "b9_comm_init: world %d > %d", world, REBALANCE_MAX_WORLD);
     int rc = load_nccl(); if (rc) return rc;
     std::lock_guard<std::mutex> in_lk(c->in_mu);
-    std::lock_guard<std::mutex> out_lk(c->out_mu);
+    OutLock out_lk(c);
     CU(cudaSetDevice(c->device));
     B9NcclId id; memcpy(id.internal, id128, 128);
     if (c->nccl_comm) { nccl_comm_destroy(c->nccl_comm); c->nccl_comm = nullptr; }   // re-init: the old communicator is not leaked
@@ -1349,7 +1402,7 @@ int b9_rebalance(b9_ctx* c, b9_rebalance_info* info) {
     if (!c) return fail(B9_EINVAL, "b9_rebalance: ctx is NULL");
     if (!c->nccl_comm) return fail(B9_EINVAL, "b9_rebalance: b9_comm_init was not called");
     std::lock_guard<std::mutex> in_lk(c->in_mu);       // the exchange rewrites both ends of the ring: no push, no drain meanwhile
-    std::lock_guard<std::mutex> out_lk(c->out_mu);
+    OutLock out_lk(c);
     std::lock_guard<std::mutex> lk(c->mu);
     CU(cudaSetDevice(c->device));
     const int W = c->comm_world, R = c->comm_rank;
@@ -1582,7 +1635,7 @@ int64_t b9_drain_fetch_object(b9_ctx* c, uint8_t* obj, uint64_t cap, uint64_t* o
     if (!c || !obj) return fail(B9_EINVAL, "b9_drain_fetch_object: NULL argument");
     uint32_t n = 0; uint64_t bytes = 0;
     {
-        std::lock_guard<std::mutex> out_lk(c->out_mu);
+        OutLock out_lk(c);
         CU(cudaSetDevice(c->device));
         { int rc = finish_launch(c); if (rc) return rc; }
         if (!c->have_results) return fail(B9_EINVAL, "b9_drain_fetch_object: no drain results are waiting");
@@ -1655,9 +1708,10 @@ int b9_stats_get(b9_ctx* c, b9_stats* out) {
 int b9_sync(b9_ctx* c) {
     if (!c) return fail(B9_EINVAL, "b9_sync: ctx is NULL");
     CU(cudaSetDevice(c->device));
+    { OutLock span_lk(c); }                    // the open span ends behind the last drain kernel, not after this wait
     CU(cudaStreamSynchronize(c->stream_in));
     CU(cudaStreamSynchronize(c->stream));
-    std::lock_guard<std::mutex> out_lk(c->out_mu);
+    OutLock out_lk(c);
     return finish_launch(c);
 }
 

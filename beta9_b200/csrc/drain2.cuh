@@ -21,7 +21,11 @@
 //     NOT walked by one lane: the warp splits the body into 32 chunks, every lane finds its first
 //     code-unit boundary by a bounded look-behind and transcodes its chunk (esc_* below);
 //   * anything that is not the SDK's canonical frame goes through the sequential validating parser
-//     (json_device.cuh) — correctness first, it is rare.
+//     (json_device.cuh) — correctness first, it is rare;
+//   * back-to-back drains overlap: a drain launched right behind another one is its programmatic dependent. Its warps
+//     copy and classify their first (static) tile while the previous grid drains out, then wait for it
+//     (griddepcontrol.wait) before the first access to the control block or the outputs. The control block comes from a
+//     ring (D3_CTL_RING) whose next entry each kernel zeroes, so no memset runs between two launches.
 //
 // Reference behaviour realised: see drain_kernel.cuh's header (pop, decode, loads, call, result).
 #pragma once
@@ -48,6 +52,10 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
     return ok != 0;
 }
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) { while (!mbar_try_wait(bar, parity)) {} }
+// programmatic dependent launch: let the next grid on the stream become resident / wait until the previous grid has
+// completed and its memory is visible (a no-op when this grid was not launched as a programmatic dependent)
+__device__ __forceinline__ void grid_dep_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+__device__ __forceinline__ void grid_dep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 // global -> shared::cta bulk async copy; dst/src 16-byte aligned, bytes a multiple of 16
 __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
@@ -1435,6 +1443,11 @@ __global__ void __launch_bounds__(D3_WARPS * 32, (HANDLER == 1 ? B9_CRC_MINB : H
     uint8_t* const sbuf = wbase + ((sizeof(D3Warp<T>) + 127u) & ~127u);   // stage buffer (+64 bytes of readable slack)
     const int k = lane / G, sub = lane % G;                                // my task inside the warp-tile, my share of it
 
+    // Back-to-back drains overlap (programmatic dependent launch, see the host's launch_drain3): the next drain's CTAs may
+    // become resident as soon as this grid's leave. Until its grid_dep_wait a warp touches only what no drain writes — slot
+    // words, ids, payload — and its own shared memory: the first tile's bulk copy and phase A. Everything an earlier drain
+    // writes (the control block, out_*, the slow list, tile_base / block_base) comes after the wait.
+    grid_dep_launch_dependents();
     if (HANDLER == 1) { for (int i = threadIdx.x; i < 256; i += D3_WARPS * 32) s_crc_table[i] = crc_table_entry(i); __syncthreads(); }
     if (HANDLER == 3) {
         for (int i = threadIdx.x; i < 256; i += D3_WARPS * 32) s_jcls[i] = json_cls_of((uint32_t)i);
@@ -1453,7 +1466,8 @@ __global__ void __launch_bounds__(D3_WARPS * 32, (HANDLER == 1 ? B9_CRC_MINB : H
     // Tile sequence of a worker: its first `static_rounds` tiles are worker + q * workers (no shared
     // counter: one L2 atomic round trip less per tile, measured 4 %); the rest of the window comes from
     // the global ticket counter, so the last rounds are still balanced by work stealing. The host sets
-    // static_rounds = 0 whenever tile costs are not uniform (cancelled slots, variable-size handlers).
+    // static_rounds = 1 whenever tile costs are not uniform (cancelled slots, variable-size handlers): a worker's
+    // first tile is always static, so that it can be copied and worked on before the grid-dependency wait.
     const unsigned long long n_workers = (unsigned long long)gridDim.x * D3_WARPS;
     const unsigned long long wid = (unsigned long long)blockIdx.x * D3_WARPS + warp;
     const unsigned long long dyn_base = (unsigned long long)a.static_rounds * n_workers;
@@ -1465,11 +1479,16 @@ __global__ void __launch_bounds__(D3_WARPS * 32, (HANDLER == 1 ? B9_CRC_MINB : H
         ++q;
         return t;
     };
-    unsigned long long t_cur = fetch(), t_raw = fetch();
-    t_cur = __shfl_sync(0xffffffffu, t_cur, 0);
+    unsigned long long t_cur = fetch(), t_raw = 0;                         // (q = 0: static on every lane)
     D3MetaRegs mregs; mregs.off = 0; mregs.hdr = 0; mregs.id = make_uint4(0u, 0u, 0u, 0u);
     if (t_cur < a.n_tiles) d3_load_meta<T>(a, t_cur, lane, mregs, TT);
     uint32_t parity = 0;
+    bool waited = false;                                                   // grid_dep_wait done (first tile: before its cursor add)
+    auto advance = [&]() {                                                 // t_cur := the tile fetched last time, its slot words in flight
+        t_cur = __shfl_sync(0xffffffffu, t_raw, 0);
+        if (t_cur < a.n_tiles) d3_load_meta<T>(a, t_cur, lane, mregs, TT);
+        t_raw = fetch();
+    };
 
     while (t_cur < a.n_tiles) {
         // ---------------- stage: decide how the tile's bytes get to shared memory, fire the copy --------
@@ -1501,13 +1520,10 @@ __global__ void __launch_bounds__(D3_WARPS * 32, (HANDLER == 1 ? B9_CRC_MINB : H
         // record indices: ready counts are known from the slot words alone
         const uint32_t ready_mask_t = __ballot_sync(0xffffffffu, m_ready);       // bit = task index
         const uint32_t rc = __popc(ready_mask_t);
-        const uint32_t base_cnt = a.count_mode ? tile_ready_before(a, tile, TT) : t0;   // (count_mode: from the pre-pass kernels)
-        if (lane == 0 && tile == a.n_tiles - 1) a.ctl->total_cnt = base_cnt + rc;
-        // advance the ticket pipeline (loads/atomics issued here are consumed one iteration later)
-        t_cur = __shfl_sync(0xffffffffu, t_raw, 0);
-        if (t_cur < a.n_tiles) d3_load_meta<T>(a, t_cur, lane, mregs, TT);
-        t_raw = fetch();
-        __syncwarp();                                                      // W.* visible to all lanes
+        // advance the ticket pipeline (loads/atomics issued here are consumed one iteration later); on the first tile
+        // the tickets touch the control block, so this waits for the grid-dependency wait below
+        if (waited) advance();
+        __syncwarp();                                                     // W.* visible to all lanes
         if (staged) { mbar_wait(&W.mbar, parity); parity ^= 1u; }
 
         // ---------------- phase A: G lanes per task ----------------------------------------------------
@@ -1645,6 +1661,16 @@ __global__ void __launch_bounds__(D3_WARPS * 32, (HANDLER == 1 ? B9_CRC_MINB : H
             }
         }
 
+        if (!waited) {                                                     // first tile: from here on the control block and out_* are used
+            grid_dep_wait();
+            waited = true;
+            if (wid == 0 && lane == 0) *a.ctl_next = DrainCtl{};          // (worker 0 always has tile 0)
+            t_raw = fetch();
+            advance();
+        }
+        const uint32_t base_cnt = a.count_mode ? tile_ready_before(a, tile, TT) : t0;   // (count_mode: from the pre-pass kernels)
+        if (lane == 0 && tile == a.n_tiles - 1) a.ctl->total_cnt = base_cnt + rc;
+
         // ---------------- compaction (ballot) + sizes (scan) + ONE cursor add per warp-tile -------------
         const uint32_t my_bytes = (sub == 0) ? rec.out_len : 0u;
         const uint32_t ex_bytes0 = warp_excl_scan(my_bytes, lane);
@@ -1703,6 +1729,7 @@ __global__ void __launch_bounds__(D3_WARPS * 32, (HANDLER == 1 ? B9_CRC_MINB : H
         // the compiler keep the whole block in local memory, and the main loop then reads its arguments with LDL — measured
         // +24 us per 1M-task drain)
         const DrainArgs tail_args = a;
+        if (!waited) grid_dep_wait();                                      // (a worker without a tile)
         d3_identity_tail(tail_args, sbuf, in_cap, lane, (uint32_t)n_workers);
     }
 }

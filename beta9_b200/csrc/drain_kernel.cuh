@@ -33,6 +33,13 @@ struct DrainCtl {
     unsigned int workers_done;      // identity: workers that are through with their tiles (everything they defer is published before)
 };
 
+// Control blocks of the drain: a ring, so that no memset has to run between two back-to-back drain kernels. Launch e uses
+// entry e % D3_CTL_RING and, after its grid-dependency wait (launch e - 1 has completed), zeroes entry (e + 1) % D3_CTL_RING
+// for launch e + 1. Two entries suffice: the entry launch e zeroes is the one launch e - 1 used, and nothing reads that one
+// any more — launch e - 1 is complete, launch e + 1 touches its own entry only after its own wait (launch e has completed,
+// zeroing included), and the host reads an entry only for the launch it finishes, which is then the last one enqueued.
+constexpr uint32_t D3_CTL_RING = 2;
+
 // A task the identity main loop could not settle. Published without a lock: w1 first, then (after a fence) w0, whose upper
 // 24 bits carry the launch's epoch — a consumer that claimed the slot polls w0 until the epoch is this launch's.
 struct SlowItem {
@@ -59,8 +66,9 @@ struct DrainArgs {
     uint8_t*  out_status;           // [n_tasks]
     uint8_t*  out_has;              // [n_tasks]
     // control
-    DrainCtl* ctl;
-    const uint32_t* tile_base;      // count_mode: [n_tiles] ready tasks before each warp-tile inside its 256-slot block (tile_count_kernel)
+    DrainCtl* ctl;                  // this launch's entry of the control ring: ctl[epoch % D3_CTL_RING]
+    DrainCtl* ctl_next;             // the next launch's entry: zeroed by this launch once the previous one has completed
+    const uint32_t* tile_base;     // count_mode: [n_tiles] ready tasks before each warp-tile inside its 256-slot block (tile_count_kernel)
     const uint32_t* block_base;     // count_mode: [n / 256 + 1] ready tasks before each 256-slot block (tile_scan_kernel); last = window total
     int handler;
     uint32_t count_mode;            // 0 = no pending task is cancelled (record index = task index), 1 = record index from tile_base
