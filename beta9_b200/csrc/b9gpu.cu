@@ -36,6 +36,10 @@
 
 #include <dlfcn.h>
 
+// wire_encode_kernel<true> for b9_wire_encode_full, launched from its own translation unit (wire_full.cu says why);
+// args: a WireArgs, env: the device copy of the WireEnv
+cudaError_t launch_wire_encode_full(const void* args, size_t args_size, const void* env, uint32_t grid, cudaStream_t s);
+
 using namespace b9;
 
 namespace {
@@ -1057,8 +1061,10 @@ static size_t host_go_quote(const char* s, uint8_t* o, size_t cap) {
     return n;
 }
 
-int64_t b9_wire_encode(b9_ctx* c, const b9_wire_env* env, uint32_t max_tasks) {
-    if (!c || !env || !env->workspace_name || !env->stub_id) return fail(B9_EINVAL, "b9_wire_encode: NULL argument");
+// b9_wire_encode (full = false) and b9_wire_encode_full: the same call around wire_encode_kernel<full>
+static int64_t wire_encode(b9_ctx* c, const b9_wire_env* env, uint32_t max_tasks, bool full) {
+    const char* const fn = full ? "b9_wire_encode_full" : "b9_wire_encode";
+    if (!c || !env || !env->workspace_name || !env->stub_id) return fail(B9_EINVAL, "%s: NULL argument", fn);
     OutLock out_lk(c);
     CU(cudaSetDevice(c->device));
     c->have_results = false; c->res_async = false; c->burst_open = false;
@@ -1082,7 +1088,7 @@ int64_t b9_wire_encode(b9_ctx* c, const b9_wire_env* env, uint32_t max_tasks) {
         lit(",\"stub_id\":");          k += host_go_quote(env->stub_id, o + std::min(k, cap), cap - std::min(k, cap));
         lit(",\"executor\":");         k += host_go_quote(env->executor ? env->executor : "taskqueue", o + std::min(k, cap), cap - std::min(k, cap));
         lit(",\"args\":");
-        if (k > cap) return fail(B9_E2BIG, "b9_wire_encode: workspace/stub names too long");
+        if (k > cap) return fail(B9_E2BIG, "%s: workspace/stub names too long", fn);
         we.mid_len = (uint32_t)k;
     }
     we.max_retries = env->max_retries; we.timeout = env->timeout; we.ttl = env->ttl;
@@ -1095,12 +1101,13 @@ int64_t b9_wire_encode(b9_ctx* c, const b9_wire_env* env, uint32_t max_tasks) {
     a.out_payload = c->d_out_payload; a.out_cap = c->max_result_bytes; a.out_off = c->d_out_off; a.out_len = c->d_out_len;
     a.out_ids = c->d_out_ids; a.out_status = c->d_out_status; a.out_has = c->d_out_has; a.ctl = c->d_ctl;
     CU(cudaEventRecord(c->ev_a, s));
-    wire_encode_kernel<<<(n + 127) / 128, 128, 0, s>>>(a, c->d_wire_env);
+    if (full) CU(launch_wire_encode_full(&a, sizeof a, c->d_wire_env, (n + 127) / 128, s));
+    else wire_encode_kernel<false><<<(n + 127) / 128, 128, 0, s>>>(a, c->d_wire_env);
     CU(cudaGetLastError());
     CU(cudaEventRecord(c->ev_b, s));
     CU(cudaMemcpyAsync(c->h_ctl, c->d_ctl, sizeof(DrainCtl), cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));     // (the stack copy of `we` is consumed by now as well)
-    if (c->h_ctl->overflow) return fail(B9_ENOSPC, "b9_wire_encode: records exceed max_result_bytes (%llu)", (unsigned long long)c->max_result_bytes);
+    if (c->h_ctl->overflow) return fail(B9_ENOSPC, "%s: records exceed max_result_bytes (%llu)", fn, (unsigned long long)c->max_result_bytes);
     c->res_bytes = c->h_ctl->bytes; c->res_n = n; c->res_popped = 0; c->have_results = true;
     float ms = 0; cudaEventElapsedTime(&ms, c->ev_a, c->ev_b); c->res_kernel_ms = ms;
     std::lock_guard<std::mutex> lk(c->mu);
@@ -1109,6 +1116,9 @@ int64_t b9_wire_encode(b9_ctx* c, const b9_wire_env* env, uint32_t max_tasks) {
     c->stats.last_drain_kernel_ms = ms;
     return (int64_t)n;
 }
+
+int64_t b9_wire_encode(b9_ctx* c, const b9_wire_env* env, uint32_t max_tasks) { return wire_encode(c, env, max_tasks, false); }
+int64_t b9_wire_encode_full(b9_ctx* c, const b9_wire_env* env, uint32_t max_tasks) { return wire_encode(c, env, max_tasks, true); }
 
 // =========================================================================== multi-GPU: NCCL rebalance
 }  // extern "C" (reopened below)

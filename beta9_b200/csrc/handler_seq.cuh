@@ -40,16 +40,50 @@ __device__ inline uint32_t py_string_write(const uint8_t* __restrict__ p, uint32
     return n + 1;
 }
 
-// json.dumps of the value Go decodes from the validated, non-empty JSON list or object p[s..e), as the runner's
-// json.loads reads it back from Go's encoding: separators ", " and ": ", strings by py_emit (ensure_ascii), numbers
-// by py_json_go_number, object members in Go's map order -- keys sorted bytewise by their decoded UTF-8, the last
-// of duplicate keys winning. That order needs no storage: each step scans the object for the smallest key after the
-// one emitted last (among equal keys the last occurrence), which is quadratic in the member count.
+// Go's encoding/json of a string token p[s..e) (quotes included, validated) as Go decoded it: go_emit per code point
+__device__ inline uint32_t go_string_len(const uint8_t* __restrict__ p, uint32_t s, uint32_t e) {
+    uint32_t i = s + 1, end = e - 1, out = 2;
+    while (i < end) out += go_emit_len(next_cp(p, i, end));
+    return out;
+}
+__device__ inline uint32_t go_string_write(const uint8_t* __restrict__ p, uint32_t s, uint32_t e, uint8_t* __restrict__ o) {
+    uint32_t i = s + 1, end = e - 1, n = 1;
+    o[0] = '"';
+    while (i < end) n += go_emit(next_cp(p, i, end), o + n);
+    o[n] = '"';
+    return n + 1;
+}
+
+// How value_json writes what the walk visits: separators, strings (token with its quotes), numbers (o == nullptr: size)
+struct PyJsonWriter {       // CPython json.dumps (ensure_ascii, separators ", " / ": ") of what json.loads makes of Go's text
+    static constexpr bool SPACED = true;
+    __device__ static __forceinline__ uint32_t string_len(const uint8_t* __restrict__ p, uint32_t s, uint32_t e) { return py_string_len(p, s, e); }
+    __device__ static __forceinline__ uint32_t string_write(const uint8_t* __restrict__ p, uint32_t s, uint32_t e, uint8_t* __restrict__ o) {
+        return py_string_write(p, s, e, o);
+    }
+    __device__ static __forceinline__ uint32_t number(unsigned long long bits, uint8_t* o) { return py_json_go_number(bits, o); }
+};
+struct GoJsonWriter {       // Go encoding/json (TaskMessage.Encode): no white space, HTML-safe strings, float64 text
+    static constexpr bool SPACED = false;
+    __device__ static __forceinline__ uint32_t string_len(const uint8_t* __restrict__ p, uint32_t s, uint32_t e) { return go_string_len(p, s, e); }
+    __device__ static __forceinline__ uint32_t string_write(const uint8_t* __restrict__ p, uint32_t s, uint32_t e, uint8_t* __restrict__ o) {
+        return go_string_write(p, s, e, o);
+    }
+    __device__ static __forceinline__ uint32_t number(unsigned long long bits, uint8_t* o) { return go_json_float(bits, o); }
+};
+
+// The value Go decodes from the validated, non-empty JSON list or object p[s..e), written by W: object members in Go's
+// map order -- keys sorted bytewise by their decoded UTF-8 (escapes resolved, invalid UTF-8 and lone surrogates as
+// U+FFFD), the last of duplicate keys winning. That order needs no storage: each step scans the object for the
+// smallest key after the one emitted last (among equal keys the last occurrence), which is quadratic in the member
+// count. drop_args: leave out the top-level object's member "args" (exact decoded key; an HTTP body's remaining map).
 // o == nullptr: size only. Returns the byte count, or -1 where the device DECLINES: nesting deeper than
 // PY_VALUE_MAX_DEPTH, an object with more than PY_VALUE_MAX_MEMBERS members, a number f64_parse cannot settle.
+// Instantiated out of line below: py_value_json (identity's result) and go_value_json (the wire record).
 constexpr int PY_VALUE_MAX_DEPTH = 16;
 constexpr uint32_t PY_VALUE_MAX_MEMBERS = 64;
-__device__ __noinline__ int64_t py_value_json(const uint8_t* __restrict__ p, uint32_t s, uint32_t e, uint8_t* __restrict__ o) {
+template <class W>
+__device__ __forceinline__ int64_t value_json(const uint8_t* __restrict__ p, uint32_t s, uint32_t e, uint8_t* __restrict__ o, bool drop_args) {
     uint32_t pos[PY_VALUE_MAX_DEPTH];              // list: the next element (or ','); object: just past its '{'
     uint32_t lks[PY_VALUE_MAX_DEPTH], lke[PY_VALUE_MAX_DEPTH];   // object: body of the key emitted last
     uint32_t is_obj = 0, started = 0;              // bit d: the container at depth d is an object / has emitted a member
@@ -72,13 +106,13 @@ __device__ __noinline__ int64_t py_value_json(const uint8_t* __restrict__ p, uin
                     if (c == '{') is_obj |= bit; else is_obj &= ~bit;
                     ++depth;
                 }
-            } else if (c == '"') n += o ? py_string_write(p, vs, ve, o + n) : py_string_len(p, vs, ve);
+            } else if (c == '"') n += o ? W::string_write(p, vs, ve, o + n) : W::string_len(p, vs, ve);
             else if (c == 't' || c == 'n') { if (o) for (int k = 0; k < 4; ++k) o[n + k] = p[vs + k]; n += 4; }
             else if (c == 'f') { if (o) for (int k = 0; k < 5; ++k) o[n + k] = p[vs + k]; n += 5; }
             else {
                 unsigned long long b = 0;
                 if (!f64_parse(p, vs, ve, &b)) return -1;
-                n += py_json_go_number(b, o ? o + n : nullptr);
+                n += W::number(b, o ? o + n : nullptr);
             }
         }
         if (depth == 0) return n;
@@ -90,7 +124,7 @@ __device__ __noinline__ int64_t py_value_json(const uint8_t* __restrict__ p, uin
             while (is_ws(p[i])) ++i;
             if (p[i] == ']') { if (o) o[n] = ']'; ++n; --depth; continue; }
             if (p[i] == ',') { ++i; while (is_ws(p[i])) ++i; }
-            if (started & bit) { if (o) { o[n] = ','; o[n + 1] = ' '; } n += 2; }
+            if (started & bit) { if (o) { o[n] = ','; if (W::SPACED) o[n + 1] = ' '; } n += W::SPACED ? 2 : 1; }
             started |= bit;
             vs = i; ve = (uint32_t)skip_value(p, i, e, f); pos[d] = ve; have = true;
             continue;
@@ -112,17 +146,26 @@ __device__ __noinline__ int64_t py_value_json(const uint8_t* __restrict__ p, uin
             i = (uint32_t)skip_value(p, i, e, f);
             if (++members > PY_VALUE_MAX_MEMBERS) return -1;
             if ((started & bit) && !key_less(p, lks[d], lke[d], ks + 1, ke - 1)) continue;   // emitted already
+            if (drop_args && d == 0 && match_exact_key(p, ks + 1, ke - 1) == 1) continue;
             if (!found || !key_less(p, bks + 1, bke - 1, ks + 1, ke - 1)) { found = true; bks = ks; bke = ke; bvs = v0; bve = i; }
         }
         if (!found) { if (o) o[n] = '}'; ++n; --depth; continue; }
-        if (started & bit) { if (o) { o[n] = ','; o[n + 1] = ' '; } n += 2; }
+        if (started & bit) { if (o) { o[n] = ','; if (W::SPACED) o[n + 1] = ' '; } n += W::SPACED ? 2 : 1; }
         started |= bit;
         lks[d] = bks + 1; lke[d] = bke - 1;
-        n += o ? py_string_write(p, bks, bke, o + n) : py_string_len(p, bks, bke);
-        if (o) { o[n] = ':'; o[n + 1] = ' '; }
-        n += 2;
+        n += o ? W::string_write(p, bks, bke, o + n) : W::string_len(p, bks, bke);
+        if (o) { o[n] = ':'; if (W::SPACED) o[n + 1] = ' '; }
+        n += W::SPACED ? 2 : 1;
         vs = bvs; ve = bve; have = true;
     }
+}
+// json.dumps of the value as the runner's json.loads reads it back from Go's encoding (identity's result)
+__device__ __noinline__ int64_t py_value_json(const uint8_t* __restrict__ p, uint32_t s, uint32_t e, uint8_t* __restrict__ o) {
+    return value_json<PyJsonWriter>(p, s, e, o, false);
+}
+// Go's json.Marshal of the value (TaskMessage.Encode's args / kwargs)
+__device__ __noinline__ int64_t go_value_json(const uint8_t* __restrict__ p, uint32_t s, uint32_t e, uint8_t* __restrict__ o, bool drop_args) {
+    return value_json<GoJsonWriter>(p, s, e, o, drop_args);
 }
 
 // Lane 0: classify args[0] for the handler and fill the record. `pr` is the parse of the payload.

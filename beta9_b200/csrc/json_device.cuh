@@ -498,4 +498,30 @@ __device__ inline uint32_t py_emit(uint32_t cp, uint8_t* __restrict__ o) {
     return nu * 6;
 }
 
+// ---- Go encoding/json string escaping (encode.go appendString, HTML-safe) -------------------------------------
+// < > & -> < > &, U+2028/9 escaped, \b \f \n \r \t short forms, other controls \u00XX, the rest raw UTF-8
+__device__ __forceinline__ uint32_t go_emit_len(uint32_t cp) {
+    if (cp < 0x80) {
+        if (cp == '"' || cp == '\\' || cp == '\b' || cp == '\f' || cp == '\n' || cp == '\r' || cp == '\t') return 2;
+        if (cp < 0x20 || cp == '<' || cp == '>' || cp == '&') return 6;
+        return 1;
+    }
+    if (cp == 0x2028 || cp == 0x2029) return 6;
+    return cp < 0x800 ? 2u : (cp < 0x10000 ? 3u : 4u);
+}
+__device__ inline uint32_t go_emit(uint32_t cp, uint8_t* __restrict__ o) {
+    if (cp < 0x80) {
+        uint8_t sc = 0;
+        switch (cp) { case '"': sc = '"'; break; case '\\': sc = '\\'; break; case '\b': sc = 'b'; break; case '\f': sc = 'f'; break;
+                      case '\n': sc = 'n'; break; case '\r': sc = 'r'; break; case '\t': sc = 't'; break; }
+        if (sc) { o[0] = '\\'; o[1] = sc; return 2; }
+        if (cp < 0x20 || cp == '<' || cp == '>' || cp == '&') { o[0] = '\\'; o[1] = 'u'; o[2] = '0'; o[3] = '0'; o[4] = hexdig(cp >> 4); o[5] = hexdig(cp & 15); return 6; }
+        o[0] = (uint8_t)cp; return 1;
+    }
+    if (cp == 0x2028 || cp == 0x2029) { o[0] = '\\'; o[1] = 'u'; o[2] = '2'; o[3] = '0'; o[4] = '2'; o[5] = (cp == 0x2028) ? '8' : '9'; return 6; }
+    if (cp < 0x800) { o[0] = 0xC0 | (cp >> 6); o[1] = 0x80 | (cp & 0x3F); return 2; }
+    if (cp < 0x10000) { o[0] = 0xE0 | (cp >> 12); o[1] = 0x80 | ((cp >> 6) & 0x3F); o[2] = 0x80 | (cp & 0x3F); return 3; }
+    o[0] = 0xF0 | (cp >> 18); o[1] = 0x80 | ((cp >> 12) & 0x3F); o[2] = 0x80 | ((cp >> 6) & 0x3F); o[3] = 0x80 | (cp & 0x3F); return 4;
+}
+
 }  // namespace b9

@@ -10,14 +10,20 @@
 // raw UTF-8), map keys sorted, no whitespace, nil Args -> [], nil Kwargs -> null, integer-valued
 // float64 printed as digits. PARITY UNPINNED like the oracle's restatement (DESIGN.md §3).
 //
-// Device domain: numbers must be plain integers of <= 15 digits (anything else needs strconv's
-// shortest-float formatting), object keys must already be in strictly increasing byte order (Go
-// would sort them). Everything else is reported B9_ST_UNSUPPORTED, never approximated.
+// Two entry points share one kernel, wire_encode_kernel<FULL>:
+//   * b9_wire_encode (FULL = false). Device domain: numbers must be plain integers of <= 15 digits (anything else
+//     needs strconv's shortest-float formatting), object keys must already be in strictly increasing byte order (Go
+//     would sort them), SDK payloads only. Everything else is reported B9_ST_UNSUPPORTED, never approximated.
+//   * b9_wire_encode_full (FULL = true): go_transcode where it answers (the copy-like path of canonical payloads),
+//     else the ordered walk go_value_json (handler_seq.cuh): every number go_json_float(f64_parse(literal)), objects
+//     in Go's map order, duplicates last-wins; HTTP bodies by SerializeHttpPayload's map rules (wire_full_values).
+//     Declines: merged struct kwargs, a literal f64_parse cannot settle, the walk's depth / member limits, TASK_MSG
+//     and PICKLE tasks.
 // One thread per task: a sizing walk, one cursor add per warp, an emitting walk.
 #pragma once
 #include <stdint.h>
 #ifdef B9_WIRE_ENCODE_HELPERS_ONLY      // tests/host_shim builds the value encoders below for the host
-#include "json_device.cuh"
+#include "handler_seq.cuh"
 #else
 #include "drain_kernel.cuh"
 #endif
@@ -29,30 +35,6 @@ struct WireEnv {
     uint8_t mid[512]; uint32_t mid_len;
     uint32_t max_retries; int32_t timeout; uint32_t ttl;
 };
-
-__device__ __forceinline__ uint32_t go_emit_len(uint32_t cp) {
-    if (cp < 0x80) {
-        if (cp == '"' || cp == '\\' || cp == '\b' || cp == '\f' || cp == '\n' || cp == '\r' || cp == '\t') return 2;
-        if (cp < 0x20 || cp == '<' || cp == '>' || cp == '&') return 6;
-        return 1;
-    }
-    if (cp == 0x2028 || cp == 0x2029) return 6;
-    return cp < 0x800 ? 2u : (cp < 0x10000 ? 3u : 4u);
-}
-__device__ inline uint32_t go_emit(uint32_t cp, uint8_t* __restrict__ o) {
-    if (cp < 0x80) {
-        uint8_t sc = 0;
-        switch (cp) { case '"': sc = '"'; break; case '\\': sc = '\\'; break; case '\b': sc = 'b'; break; case '\f': sc = 'f'; break;
-                      case '\n': sc = 'n'; break; case '\r': sc = 'r'; break; case '\t': sc = 't'; break; }
-        if (sc) { o[0] = '\\'; o[1] = sc; return 2; }
-        if (cp < 0x20 || cp == '<' || cp == '>' || cp == '&') { o[0] = '\\'; o[1] = 'u'; o[2] = '0'; o[3] = '0'; o[4] = hexdig(cp >> 4); o[5] = hexdig(cp & 15); return 6; }
-        o[0] = (uint8_t)cp; return 1;
-    }
-    if (cp == 0x2028 || cp == 0x2029) { o[0] = '\\'; o[1] = 'u'; o[2] = '2'; o[3] = '0'; o[4] = '2'; o[5] = (cp == 0x2028) ? '8' : '9'; return 6; }
-    if (cp < 0x800) { o[0] = 0xC0 | (cp >> 6); o[1] = 0x80 | (cp & 0x3F); return 2; }
-    if (cp < 0x10000) { o[0] = 0xE0 | (cp >> 12); o[1] = 0x80 | ((cp >> 6) & 0x3F); o[2] = 0x80 | (cp & 0x3F); return 3; }
-    o[0] = 0xF0 | (cp >> 18); o[1] = 0x80 | ((cp >> 12) & 0x3F); o[2] = 0x80 | ((cp >> 6) & 0x3F); o[3] = 0x80 | (cp & 0x3F); return 4;
-}
 
 // Re-encode the validated JSON value p[s..e) by Go's rules. o == nullptr: size only.
 // Returns the byte count, or -1 if the value is outside the device domain.
@@ -114,6 +96,54 @@ __device__ inline int64_t go_transcode(const uint8_t* __restrict__ p, uint32_t s
     }
     return n;
 }
+
+// ---- b9_wire_encode_full: what TaskMessage.Encode writes for Args and Kwargs ----------------------------------
+// How one of the two values is written: a span of the payload (go_transcode, or the ordered walk), or a constant.
+enum GoValMode : uint8_t { GV_TRANSCODE = 0, GV_WALK, GV_WALK_NO_ARGS /* an HTTP body's map minus "args" */,
+                           GV_LIST_NIL /* [] */, GV_MAP_NIL /* null */, GV_MAP_EMPTY /* {} */ };
+struct GoVal { uint32_t s, e; int64_t len; uint8_t mode; };
+
+// Sizes the value p[s..e): go_transcode where it answers, the walk where it declines. len < 0: the walk declines too.
+__device__ inline GoVal go_val_plan(const uint8_t* __restrict__ p, uint32_t s, uint32_t e, bool drop_args) {
+    GoVal v; v.s = s; v.e = e; v.len = -1; v.mode = drop_args ? GV_WALK_NO_ARGS : GV_TRANSCODE;
+    if (!drop_args) v.len = go_transcode(p, s, e, nullptr);
+    if (v.len < 0) { if (!drop_args) v.mode = GV_WALK; v.len = go_value_json(p, s, e, nullptr, drop_args); }
+    return v;
+}
+__device__ inline GoVal go_val_const(uint8_t mode) { GoVal v; v.s = v.e = 0; v.mode = mode; v.len = mode == GV_MAP_NIL ? 4 : 2; return v; }
+
+// Writes what go_val_plan sized: exactly v.len bytes.
+__device__ inline uint32_t go_val_write(const uint8_t* __restrict__ p, const GoVal& v, uint8_t* __restrict__ o) {
+    switch (v.mode) {
+    case GV_TRANSCODE: return (uint32_t)go_transcode(p, v.s, v.e, o);
+    case GV_WALK: case GV_WALK_NO_ARGS: return (uint32_t)go_value_json(p, v.s, v.e, o, v.mode == GV_WALK_NO_ARGS);
+    case GV_LIST_NIL: o[0] = '['; o[1] = ']'; return 2;
+    case GV_MAP_NIL: o[0] = 'n'; o[1] = 'u'; o[2] = 'l'; o[3] = 'l'; return 4;
+    default: o[0] = '{'; o[1] = '}'; return 2;
+    }
+}
+
+// Args and Kwargs of a payload the parser accepted (pr.status == ST_OK; pr = parse_payload(p, n, http)), as
+// TaskMessage.Encode writes them. Returns false where the device declines: struct kwargs objects Go merges
+// (pr.kw_merged), or a value the walk declines.
+//   SDK payload (struct decode into TaskPayload): nil Args -> [], nil Kwargs -> null.
+//   HTTP body (SerializeHttpPayload, pkg/task/serialize.go:16-101): Args = the last "args" if it is a list, else nil
+//   ([]). Kwargs is never nil: the last "kwargs" if it is an object; otherwise the body's remaining map -- the whole
+//   top-level object minus "args" when that was taken as Args; {} for an empty or null body.
+__device__ inline bool wire_full_values(const uint8_t* __restrict__ p, uint32_t n, bool http, const Parsed& pr, GoVal& a, GoVal& k) {
+    if (pr.kw_merged) return false;
+    a = pr.args_len ? go_val_plan(p, pr.args_off, pr.args_off + pr.args_len, false) : go_val_const(GV_LIST_NIL);
+    if (pr.kw_len) k = go_val_plan(p, pr.kw_off, pr.kw_off + pr.kw_len, false);
+    else if (!http) k = go_val_const(GV_MAP_NIL);
+    else {
+        uint32_t s = 0, e = n;
+        while (s < e && is_ws(p[s])) ++s;
+        while (e > s && is_ws(p[e - 1])) --e;
+        k = (s == e || p[s] == 'n') ? go_val_const(GV_MAP_EMPTY) : go_val_plan(p, s, e, pr.args_len != 0);
+    }
+    return a.len >= 0 && k.len >= 0;
+}
+
 __device__ __forceinline__ void civil_from_days_dev(long long z, long long* y, int* m, int* d) {
     z += 719468;
     const long long era = (z >= 0 ? z : z - 146096) / 146097;
@@ -168,6 +198,8 @@ struct WireArgs {
     DrainCtl* ctl;
 };
 
+// FULL = false: b9_wire_encode; FULL = true: b9_wire_encode_full (the header comment above), instantiated in wire_full.cu
+template <bool FULL>
 __global__ void __launch_bounds__(128) wire_encode_kernel(WireArgs a, const WireEnv* __restrict__ envp) {
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     const int lane = threadIdx.x & 31;
@@ -178,20 +210,32 @@ __global__ void __launch_bounds__(128) wire_encode_kernel(WireArgs a, const Wire
     const uint8_t* p = nullptr;
     uint32_t slot = 0; uint64_t h = 0;
     int64_t la = 2, lk = 4;                      // "[]" / "null"
+    GoVal ga, gk;                                // FULL: how args / kwargs are written
     uint8_t tail[96]; uint32_t tail_len = 0;     // ,"policy":{…},"retries":N,"timestamp":N}
     if (valid) {
         slot = (uint32_t)((a.first_task + t) & a.slot_mask);
         h = a.hdr[slot];
         p = a.payload + a.off[slot];
-        pr = parse_payload(p, hdr_len(h));
-        status = pr.status;
-        if (hdr_flags(h) & B9_TF_HTTP_BODY_BIT) status = ST_UNSUPPORTED;     // an HTTP body's TaskPayload follows the map rules: not encoded here
-        if (hdr_flags(h) & B9_TF_TASK_MSG_BIT) status = ST_UNSUPPORTED;      // already a record: nothing to encode
-        if (status == ST_OK) {
-            if (pr.kw_merged) status = ST_UNSUPPORTED;                       // Go merges duplicate kwargs maps
-            if (pr.args_len) la = go_transcode(p, pr.args_off, pr.args_off + pr.args_len, nullptr);
-            if (pr.kw_len) lk = go_transcode(p, pr.kw_off, pr.kw_off + pr.kw_len, nullptr);
-            if (la < 0 || lk < 0) status = ST_UNSUPPORTED;
+        if (FULL) {
+            const bool http = (hdr_flags(h) & B9_TF_HTTP_BODY_BIT) != 0;
+            pr = parse_payload(p, hdr_len(h), http);
+            status = pr.status;
+            if (hdr_flags(h) & (B9_TF_TASK_MSG_BIT | B9_TF_PICKLE_BIT)) status = ST_UNSUPPORTED;   // a record already / not JSON
+            if (status == ST_OK) {
+                if (!wire_full_values(p, hdr_len(h), http, pr, ga, gk)) status = ST_UNSUPPORTED;
+                la = ga.len; lk = gk.len;
+            }
+        } else {
+            pr = parse_payload(p, hdr_len(h));
+            status = pr.status;
+            if (hdr_flags(h) & B9_TF_HTTP_BODY_BIT) status = ST_UNSUPPORTED;     // an HTTP body's TaskPayload follows the map rules: not encoded here
+            if (hdr_flags(h) & B9_TF_TASK_MSG_BIT) status = ST_UNSUPPORTED;      // already a record: nothing to encode
+            if (status == ST_OK) {
+                if (pr.kw_merged) status = ST_UNSUPPORTED;                       // Go merges duplicate kwargs maps
+                if (pr.args_len) la = go_transcode(p, pr.args_off, pr.args_off + pr.args_len, nullptr);
+                if (pr.kw_len) lk = go_transcode(p, pr.kw_off, pr.kw_off + pr.kw_len, nullptr);
+                if (la < 0 || lk < 0) status = ST_UNSUPPORTED;
+            }
         }
         if (status == ST_OK) {
             // the tail is small and per task: build it once in registers/local memory
@@ -243,10 +287,16 @@ __global__ void __launch_bounds__(128) wire_encode_kernel(WireArgs a, const Wire
         }
     }
     for (uint32_t k = 0; k < env.mid_len; ++k) *o++ = env.mid[k];
-    if (pr.args_len) o += go_transcode(p, pr.args_off, pr.args_off + pr.args_len, o); else { *o++ = '['; *o++ = ']'; }
     const char K0[] = ",\"kwargs\":";
-    for (int k = 0; k < 10; ++k) *o++ = (uint8_t)K0[k];
-    if (pr.kw_len) o += go_transcode(p, pr.kw_off, pr.kw_off + pr.kw_len, o); else { *o++ = 'n'; *o++ = 'u'; *o++ = 'l'; *o++ = 'l'; }
+    if (FULL) {
+        o += go_val_write(p, ga, o);
+        for (int k = 0; k < 10; ++k) *o++ = (uint8_t)K0[k];
+        o += go_val_write(p, gk, o);
+    } else {
+        if (pr.args_len) o += go_transcode(p, pr.args_off, pr.args_off + pr.args_len, o); else { *o++ = '['; *o++ = ']'; }
+        for (int k = 0; k < 10; ++k) *o++ = (uint8_t)K0[k];
+        if (pr.kw_len) o += go_transcode(p, pr.kw_off, pr.kw_off + pr.kw_len, o); else { *o++ = 'n'; *o++ = 'u'; *o++ = 'l'; *o++ = 'l'; }
+    }
     for (uint32_t k = 0; k < tail_len; ++k) *o++ = tail[k];
     const char E0[] = ",\"expires\":\"";
     for (int k = 0; k < 12; ++k) *o++ = (uint8_t)E0[k];

@@ -220,10 +220,12 @@ class DeviceQueue:
         return self._check(self._lib.b9_drain(self._ctx, HANDLERS[handler], max_tasks, C.byref(res)))
 
     def wire_encode(self, workspace_name: str, stub_id: str, max_tasks: int = 1 << 22, executor: str = "taskqueue",
-                    max_retries: int = 3, timeout: int = 3600, ttl: int = 7200) -> DrainResult:
-        """TaskMessage.Encode (pkg/types/task.go:79-90) of the pending tasks, on the device; they stay pending."""
+                    max_retries: int = 3, timeout: int = 3600, ttl: int = 7200, full: bool = False) -> DrainResult:
+        """TaskMessage.Encode (pkg/types/task.go:79-90) of the pending tasks, on the device; they stay pending.
+        full=True: b9_wire_encode_full (floats, unsorted / duplicate keys, HTTP bodies; include/b9gpu.h)."""
         env = L.WireEnv(workspace_name.encode(), stub_id.encode(), executor.encode(), max_retries, timeout, ttl)
-        n = self._check(self._lib.b9_wire_encode(self._ctx, C.byref(env), max_tasks))
+        fn = self._lib.b9_wire_encode_full if full else self._lib.b9_wire_encode
+        n = self._check(fn(self._ctx, C.byref(env), max_tasks))
         return self._fetch(n, None)
 
     # ---- multi-GPU (one DeviceQueue per rank / GPU)

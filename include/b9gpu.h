@@ -306,6 +306,19 @@ typedef struct b9_wire_env {
 } b9_wire_env;
 int64_t  b9_wire_encode(b9_ctx *ctx, const b9_wire_env *env, uint32_t max_tasks);
 
+/* b9_wire_encode_full: the same call (the first max_tasks pending tasks stay pending, record i = pending task i, fetched with
+ * b9_drain_fetch, a drain-side call, B9_ENOSPC when the records exceed max_result_bytes), over a wider domain: every number is
+ * written as Go's float64 text of strconv.ParseFloat's value (1.0 -> 1, 1e21 -> 1e+21, 12345678901234567890 ->
+ * 12345678901234567000), every object in Go's map order (keys sorted by their decoded UTF-8, the last of duplicate keys
+ * winning), and B9_TF_HTTP_BODY tasks by SerializeHttpPayload's map rules: Args = the last "args" if it is a list, else nil
+ * ([]); Kwargs = the last "kwargs" if it is an object, else the body's remaining map (the top-level object minus "args" when
+ * that was taken as Args; {} for an empty or null body). Status 0 = bytes present, 3 = Go refuses the payload (for an HTTP
+ * body: HTTP 400), 4 = declined, and only for: repeated struct "kwargs" objects that Go merges; a number literal of more than
+ * 19 significant digits whose rounding the device cannot settle; nesting deeper than 16 or an object of more than 64
+ * members; TASK_MSG and PICKLE tasks. Wherever b9_wire_encode answers, the bytes are the same. Added without an ABI version
+ * change: probe for it with dlsym. */
+int64_t  b9_wire_encode_full(b9_ctx *ctx, const b9_wire_env *env, uint32_t max_tasks);
+
 /* ---- multi-GPU: one ctx (= one process, one GPU) per rank of a box -------------------------------
  * The pending ring is sharded over the ranks; tasks are independent units (SURVEY.md §8e), so the
  * drain needs no collective. When ingest landed unevenly, b9_rebalance moves pending tasks so that
