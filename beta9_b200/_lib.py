@@ -14,6 +14,7 @@ ST_COMPLETE, ST_ERROR, ST_RETRY, ST_REJECTED, ST_UNSUPPORTED = 0, 1, 2, 3, 4
 TF_CANCELLED = 0x01
 TF_HTTP_BODY, TF_PICKLE, TF_TASK_MSG = 0x02, 0x04, 0x08
 CANCEL_MARKED, CANCEL_ALREADY, CANCEL_CLAIMED = 0x01, 0x02, 0x04      # b9_cancel outcome bits
+DRAIN_PEEK, DRAIN_ASYNC, DRAIN_PICKLE_FULL = 1, 2, 4                   # b9_drain_launch flags
 
 
 class Opts(C.Structure):

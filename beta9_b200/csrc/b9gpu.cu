@@ -39,6 +39,8 @@
 // wire_encode_kernel<true> for b9_wire_encode_full, launched from its own translation unit (wire_full.cu says why);
 // args: a WireArgs, env: the device copy of the WireEnv
 cudaError_t launch_wire_encode_full(const void* args, size_t args_size, const void* env, uint32_t grid, cudaStream_t s);
+// pickle_pass_kernel for B9_DRAIN_PICKLE_FULL, from function_drain.cu; args: the drain's DrainArgs
+cudaError_t launch_pickle_pass(const void* args, size_t args_size, int handler, int sm_count, cudaStream_t s);
 
 using namespace b9;
 
@@ -66,6 +68,7 @@ struct Segment {             // one push = one contiguous byte range of the payl
     cudaEvent_t ready;           // recorded on the ingest stream once the batch is fully on the device
     uint32_t max_len = 0;        // longest task of the batch (0 = not known: tasks that arrived in a rebalance)
     bool drain_waited = false;   // a drain launch has made the drain stream wait for `ready` (stream order covers later launches)
+    uint32_t n_pickle = 0;       // tasks of the batch carrying B9_TF_PICKLE (all of them when not known: a rebalance)
 };
 
 constexpr uint64_t RING_SLACK = 256;   // readable bytes past the ring end (vector loads may over-read)
@@ -231,7 +234,9 @@ template <int H> uint32_t drain3_warp_stride(uint32_t in_cap) {
 // overlap: the drain stream's last operation is a drain3_kernel and the window has no cancelled slot (so no count kernels
 // run first): the kernel is launched as that one's programmatic dependent — its CTAs become resident as the previous
 // grid's leave, and it waits for that grid's completion (griddepcontrol.wait) before it touches anything a drain writes
-template <int H> cudaError_t launch_drain3(DrainArgs a, uint64_t avg_task_bytes, uint32_t max_task_len, uint32_t cap_override, int sm_count, bool overlap, cudaStream_t s, int* grid_out) {
+// *tt_out: the launch's tasks per warp-tile (a count-mode record index depends on it)
+template <int H> cudaError_t launch_drain3(DrainArgs a, uint64_t avg_task_bytes, uint32_t max_task_len, uint32_t cap_override, int sm_count, bool overlap, cudaStream_t s, int* grid_out,
+                                           uint32_t* tt_out) {
     constexpr int T = D3Cfg<H>::T;
     static const bool tight = !(getenv("B9_STAGE_TIGHT") && atoi(getenv("B9_STAGE_TIGHT")) == 0);      // (=0: the A/B switch)
     uint32_t in_cap = 0, stride = 0; size_t smem = 0; int per_sm = 0;
@@ -268,6 +273,7 @@ template <int H> cudaError_t launch_drain3(DrainArgs a, uint64_t avg_task_bytes,
         if (e != cudaSuccess) return e;
     }
     a.tile_tasks = tt;
+    *tt_out = tt;
     a.n_tiles = (a.n_tasks + tt - 1) / tt;
     const uint32_t ctas_needed = (a.n_tiles + D3_WARPS - 1) / D3_WARPS;
     const int grid = (int)std::min<uint32_t>(ctas_needed, (uint32_t)(per_sm * sm_count));
@@ -541,7 +547,7 @@ static int push_impl(b9_ctx* c, const uint8_t* task_ids, const uint8_t* payload,
     // the O(n) host-side validation of the index below runs while the bytes are already on the wire
     if (bytes) CU(cudaMemcpyAsync(c->d_payload + start, payload + offsets[0], bytes, cudaMemcpyHostToDevice, s));
     uint64_t n_cancelled = 0;
-    uint32_t seg_max_len = 0;
+    uint32_t seg_max_len = 0, n_pickle = 0;
     {
         const uint32_t maxb = c->max_task_bytes;
         uint64_t bad = ~0ull, big = ~0ull, prev = offsets[0], longest = 0;
@@ -559,7 +565,10 @@ static int push_impl(b9_ctx* c, const uint8_t* task_ids, const uint8_t* payload,
             return fail(B9_E2BIG, "b9_batch_push: task %llu is %llu bytes, max_task_bytes is %u", (unsigned long long)big,
                         (unsigned long long)(offsets[big + 1] - offsets[big]), maxb);
         }
-        if (meta && meta->flags) for (uint32_t i = 0; i < n; ++i) n_cancelled += (meta->flags[i] & B9_TF_CANCELLED) ? 1 : 0;
+        if (meta && meta->flags) for (uint32_t i = 0; i < n; ++i) {
+            n_cancelled += (meta->flags[i] & B9_TF_CANCELLED) ? 1 : 0;
+            n_pickle += (meta->flags[i] & B9_TF_PICKLE) ? 1 : 0;
+        }
     }
     CU(cudaMemcpyAsync(c->d_in_off, offsets, ((size_t)n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
     // ids go straight into their ring slots (two pieces when the slot ring wraps)
@@ -584,6 +593,7 @@ static int push_impl(b9_ctx* c, const uint8_t* task_ids, const uint8_t* payload,
     {
         std::lock_guard<std::mutex> lk(c->mu);
         c->segs.push_back(Segment{tail, n, start, bytes, ready, seg_max_len});
+        c->segs.back().n_pickle = n_pickle;
         c->write_pos = start + b9_seg_span(bytes);
         c->tail_task += n;
         c->pending_bytes += bytes;
@@ -895,6 +905,7 @@ int64_t b9_drain_launch(b9_ctx* c, int handler, uint32_t max_tasks, int peek) {
     struct Piece { Segment sg; uint64_t a, b; bool wait; };
     std::vector<Piece> pieces;
     uint64_t head = 0; uint32_t n = 0; uint32_t count_mode = 0;
+    bool win_pickle = false;                                                // a B9_TF_PICKLE task may be in the window
     {
         std::lock_guard<std::mutex> lk(c->mu);
         head = c->head_task;
@@ -905,7 +916,7 @@ int64_t b9_drain_launch(b9_ctx* c, int handler, uint32_t max_tasks, int peek) {
         const uint64_t lo = head, hi = head + n;
         for (Segment& sg : c->segs) {
             const uint64_t a = std::max<uint64_t>(lo, sg.first_task), b = std::min<uint64_t>(hi, sg.first_task + sg.n);
-            if (a < b) { pieces.push_back(Piece{sg, a, b, !sg.drain_waited}); sg.drain_waited = true; }
+            if (a < b) { pieces.push_back(Piece{sg, a, b, !sg.drain_waited}); sg.drain_waited = true; win_pickle |= sg.n_pickle != 0; }
         }
     }
     if (n == 0) { c->have_results = true; return 0; }
@@ -954,18 +965,29 @@ int64_t b9_drain_launch(b9_ctx* c, int handler, uint32_t max_tasks, int peek) {
     const bool overlap = c->last_op_drain;
     c->last_op_drain = false;
     cudaError_t le;
+    uint32_t tt = 0;
     switch (handler) {
-    case B9_H_IDENTITY: le = launch_drain3<0>(a, in_bytes / n, win_max_len, c->stage_bytes_override, c->sm_count, overlap, s, &grid); break;
-    case B9_H_CRC32:    le = launch_drain3<1>(a, in_bytes / n, win_max_len, c->stage_bytes_override, c->sm_count, overlap, s, &grid); break;
-    case B9_H_VADD_F32: le = launch_drain3<2>(a, in_bytes / n, win_max_len, c->stage_bytes_override, c->sm_count, overlap, s, &grid); break;
-    default:            le = launch_drain3<3>(a, in_bytes / n, win_max_len, c->stage_bytes_override, c->sm_count, overlap, s, &grid); break;
+    case B9_H_IDENTITY: le = launch_drain3<0>(a, in_bytes / n, win_max_len, c->stage_bytes_override, c->sm_count, overlap, s, &grid, &tt); break;
+    case B9_H_CRC32:    le = launch_drain3<1>(a, in_bytes / n, win_max_len, c->stage_bytes_override, c->sm_count, overlap, s, &grid, &tt); break;
+    case B9_H_VADD_F32: le = launch_drain3<2>(a, in_bytes / n, win_max_len, c->stage_bytes_override, c->sm_count, overlap, s, &grid, &tt); break;
+    default:            le = launch_drain3<3>(a, in_bytes / n, win_max_len, c->stage_bytes_override, c->sm_count, overlap, s, &grid, &tt); break;
     }
     if (le != cudaSuccess) { c->ctl_dirty = true; return fail(B9_EIO, "drain kernel launch failed: %s", cudaGetErrorString(le)); }
     c->last_op_drain = true;
     c->burst_open = true;
+    // the function path beyond identity's one-str template: a pass over the window's pickle tasks that rewrites the records
+    // drain3_kernel left UNSUPPORTED. The next drain kernel waits for it in full (no programmatic dependent launch), and
+    // the timed span ends behind it.
+    const bool pickle_pass = (peek & B9_DRAIN_PICKLE_FULL) && win_pickle;
+    if (pickle_pass) {
+        a.tile_tasks = tt;
+        le = launch_pickle_pass(&a, sizeof a, handler, c->sm_count, s);
+        if (le != cudaSuccess) { c->last_op_drain = false; c->ctl_dirty = true; return fail(B9_EIO, "pickle pass launch failed: %s", cudaGetErrorString(le)); }
+        end_drain_span(c);
+    }
     {
         std::lock_guard<std::mutex> lk(c->mu);
-        c->stats.kernel_launches += a.count_mode ? 3 : 1;                  // (+ tile_count_kernel and tile_scan_kernel)
+        c->stats.kernel_launches += (a.count_mode ? 3 : 1) + (pickle_pass ? 1 : 0);   // (+ tile_count_kernel and tile_scan_kernel)
         c->stats.last_drain_tiles = (n + 127) / 128;                       // (reported in units of 128 tasks)
         c->stats.drains++;
     }
@@ -1596,6 +1618,7 @@ int b9_rebalance(b9_ctx* c, b9_rebalance_info* info) {
         else CU(cudaEventCreateWithFlags(&ready, cudaEventDisableTiming));
         CU(cudaEventRecord(ready, s));
         c->segs.push_back(Segment{c->tail_task, (uint32_t)rk, start, pb, ready, 0u});
+        c->segs.back().n_pickle = (uint32_t)rk;
         c->write_pos = start + b9_seg_span(pb);
         c->tail_task += rk; c->pending_bytes += pb;
     }

@@ -831,7 +831,6 @@ __device__ __forceinline__ void d3_load_meta(const DrainArgs& a, unsigned long l
 // record index base of a tile = its in-block prefix + its block's prefix (two loads in the drain).
 // (An earlier version chained the counts through a decoupled look-back inside the drain: 0.32 ms instead of 0.18 ms
 // for 1M tasks as soon as ONE slot of the window was cancelled.)
-constexpr uint32_t TC_SLOTS = 256;             // slots per tile_count_kernel block (8 warps x 32)
 __global__ void __launch_bounds__(TC_SLOTS) tile_count_kernel(const uint64_t* __restrict__ hdr, uint32_t slot_mask, uint64_t first_task, uint32_t n_tasks,
                                                               uint32_t T, uint32_t* __restrict__ base /* [n_tiles]: ready tasks before the tile, inside its block */,
                                                               uint32_t* __restrict__ block_tot /* [blocks + 1], entry b + 1 = ready tasks of block b */) {
@@ -874,10 +873,6 @@ __global__ void __launch_bounds__(1024) tile_scan_kernel(uint32_t* __restrict__ 
     __syncthreads();
     uint32_t run = s_warp[warp] + inc - sum;                              // ready tasks before my first block
     for (uint32_t i = lo; i < hi; ++i) { run += block_tot[i + 1u]; block_tot[i + 1u] = run; }
-}
-// ready tasks before warp-tile `tile` (of T slots)
-__device__ __forceinline__ uint32_t tile_ready_before(const DrainArgs& a, unsigned long long tile, uint32_t T) {
-    return __ldg(a.tile_base + tile) + __ldg(a.block_base + (uint32_t)((tile * T) / TC_SLOTS));
 }
 
 // scattered tile (it spans pushes): one bulk copy per task, each widened to 16-byte boundaries

@@ -79,6 +79,12 @@ struct DrainArgs {
     uint32_t tile_tasks;            // json_sum: tasks per warp-tile of THIS launch (4 or 8: small windows balance better on finer tiles); others: fixed
 };
 
+constexpr uint32_t TC_SLOTS = 256;             // slots per tile_count_kernel block (8 warps x 32)
+// count_mode: ready tasks before warp-tile `tile` (of T slots) — the record index of its first ready task
+__device__ __forceinline__ uint32_t tile_ready_before(const DrainArgs& a, unsigned long long tile, uint32_t T) {
+    return __ldg(a.tile_base + tile) + __ldg(a.block_base + (uint32_t)((tile * T) / TC_SLOTS));
+}
+
 __device__ __forceinline__ uint64_t ld_volatile_u64(const uint64_t* p) { return *(const volatile uint64_t*)p; }
 __device__ __forceinline__ void st_volatile_u64(uint64_t* p, uint64_t v) { *(volatile uint64_t*)p = v; }
 

@@ -172,14 +172,16 @@ class DeviceQueue:
         return marked, outcome[:n]
 
     # ---- consumer side
-    def drain(self, handler: str, max_tasks: int = 1 << 22, cap_bytes: Optional[int] = None) -> DrainResult:
+    def drain(self, handler: str, max_tasks: int = 1 << 22, cap_bytes: Optional[int] = None, full_pickle: bool = False) -> DrainResult:
+        """full_pickle=True (B9_DRAIN_PICKLE_FULL): pickle-framed tasks of every handler over plain values (include/b9gpu.h)."""
         h = HANDLERS[handler]
-        n = self._check(self._lib.b9_drain_launch(self._ctx, h, max_tasks, 0))
+        n = self._check(self._lib.b9_drain_launch(self._ctx, h, max_tasks, L.DRAIN_PICKLE_FULL if full_pickle else 0))
         return self._fetch(n, cap_bytes)
 
-    def drain_launch(self, handler: str, max_tasks: int = 1 << 22, peek: bool = False, wait: bool = True) -> int:
+    def drain_launch(self, handler: str, max_tasks: int = 1 << 22, peek: bool = False, wait: bool = True, full_pickle: bool = False) -> int:
         """wait=False (B9_DRAIN_ASYNC): returns once the kernels are enqueued; `sync()` or `fetch()` completes it."""
-        return self._check(self._lib.b9_drain_launch(self._ctx, HANDLERS[handler], max_tasks, (1 if peek else 0) | (0 if wait else 2)))
+        flags = (1 if peek else 0) | (0 if wait else 2) | (L.DRAIN_PICKLE_FULL if full_pickle else 0)
+        return self._check(self._lib.b9_drain_launch(self._ctx, HANDLERS[handler], max_tasks, flags))
 
     def fetch(self, cap_bytes: Optional[int] = None) -> DrainResult:
         self.sync()                                  # completes a wait=False launch: its byte count sizes the buffers below

@@ -9,7 +9,8 @@ reference's cloudpickle framing, routed through the batch C ABI instead of one c
 
 Every input becomes one task whose payload is exactly the bytes the reference sends (pushed with B9_TF_PICKLE); results
 come back as the bytes the reference's runner would have set and are unpickled here like `_call_remote` does. The device
-settles the shape the configurations use (one `str` argument, identity); other pickles come back UNSUPPORTED — there is no
+settles the shape the configurations use (one `str` argument, identity), and with `Function(full_pickle=True)` every
+handler over plain values (B9_DRAIN_PICKLE_FULL, include/b9gpu.h); other pickles come back UNSUPPORTED — there is no
 CPU fallback in this package: their inputs are listed in `.unsupported` for the host to route through the reference loop.
 """
 from __future__ import annotations
@@ -34,11 +35,12 @@ class Function:
 
     def __init__(self, cpu: Any = 1.0, memory: Any = 128, gpu: Any = "", image: Any = None, timeout: int = 3600, retries: int = 3,
                  name: Optional[str] = None, headless: bool = False, gpu_handler: Optional[str] = None, device: int = 0,
-                 queue: Optional[DeviceQueue] = None, **kwargs: Any):
+                 queue: Optional[DeviceQueue] = None, full_pickle: bool = False, **kwargs: Any):
         self.cpu, self.memory, self.gpu, self.image, self.timeout, self.retries = cpu, memory, gpu, image, timeout, retries
         self.name, self.headless = name, headless
         self.gpu_handler = gpu_handler or os.environ.get("B9_GPU_HANDLER", "identity")
         self.device = device
+        self.full_pickle = full_pickle            # B9_DRAIN_PICKLE_FULL: every handler over plain values, not just one str
         self.extra = kwargs
         self._queue = queue
         self.stub_id = str(uuid.uuid4())
@@ -103,7 +105,7 @@ class _CallableWrapper:
         out: List[Optional[Tuple[str, Optional[bytes]]]] = [None] * n
         seen = 0
         while seen < n:
-            r = q.drain(self.parent.gpu_handler)
+            r = q.drain(self.parent.gpu_handler, full_pickle=self.parent.full_pickle)
             if r.n == 0:
                 break
             for i in range(r.n):

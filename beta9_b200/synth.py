@@ -318,6 +318,17 @@ def values_batch(n: int, seed: int = SEED, name: str = "identity_values") -> Bat
     return _pack(chunks, lens, task_ids(n, seed), name)
 
 
+def function_docs_batch(n: int, doc_bytes: int = 1024, seed: int = SEED, name: str = "function_json_sum") -> Batch:
+    """configs[4]'s documents (json_batch) as `.map()` sends them on the function path: one cloudpickle blob
+    {"args": (doc,), "kwargs": {}} per document (sdk/src/beta9/abstractions/function.py:198-205, 246-262)."""
+    import cloudpickle
+    b = json_batch(n, doc_bytes, seed)
+    raw = b.payload.tobytes()
+    chunks = [cloudpickle.dumps({"args": (json.loads(raw[int(b.offsets[i]):int(b.offsets[i + 1])])["args"][0],), "kwargs": {}})
+              for i in range(n)]
+    return _pack(chunks, np.array([len(c) for c in chunks], dtype=np.uint64), task_ids(n, seed), name)
+
+
 def concat(batches: List[Batch]) -> Batch:
     ids = np.concatenate([b.task_ids for b in batches])
     payload = np.concatenate([b.payload for b in batches])

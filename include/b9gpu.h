@@ -101,7 +101,25 @@ enum b9_status {
                                   (pkg/abstractions/function/task.go:84,104-108); the result bytes are cloudpickle.dumps(result)
                                   (sdk/src/beta9/runner/function.py:236-283). The device settles ONE shape bit-exactly — a single
                                   `str` argument (< 64 KiB of UTF-8), no keyword arguments, handler identity — and reports every
-                                  other pickle B9_ST_UNSUPPORTED for the host's CPU loop.                                      */
+                                  other pickle B9_ST_UNSUPPORTED for the host's CPU loop.
+                                  With B9_DRAIN_PICKLE_FULL the drain also answers, bit-exactly against cloudpickle 3.1.2 on
+                                  CPython 3.12, every handler over plain values: the blob may hold PROTO 5, FRAME, EMPTY_DICT /
+                                  LIST / TUPLE, MARK, TUPLE1/2/3, TUPLE, APPEND(S), SETITEM(S), MEMOIZE, (LONG_)BINGET, str and
+                                  bytes opcodes, BININT1/2, BININT, LONG1, BINFLOAT, NONE, NEWTRUE / NEWFALSE and STOP. Call
+                                  rules: args = payload.get("args") or [], kwargs = payload.get("kwargs") or {} minus
+                                  "callback_url"; B9_ST_ERROR when args is a list / tuple of length != 1 or kwargs keeps a
+                                  member. identity: cloudpickle.dumps of the loaded value (shared objects and CPython's str
+                                  singletons stay shared); crc32: a str argument; vadd_f32: a str or bytes argument;
+                                  json_sum: sum(obj["values"]) over a list / tuple of ints, bools and floats. Every COMPLETE
+                                  has result bytes (a falsy result too). Still B9_ST_UNSUPPORTED: any other opcode (globals,
+                                  reduce, sets, bytearray, ...); a truncated or ill-formed stream; str bytes that are not UTF-8
+                                  under "surrogatepass"; a list or dict mutated after it was placed in a container or fetched
+                                  from the memo (cycles); a dict key that is not str / bytes / int / bool / float / None, a
+                                  dict of more than 64 members, or (identity) two keys equal under ==; truthy args that is
+                                  neither a list nor a tuple; json_sum's "values" of another type, or an int outside the C long
+                                  range; a result pickle of 64 KiB or more (the pickler's frame target); containers nested
+                                  deeper than 16; more than 2048 values, 2048 container members, 256 member runs, 1024 memo
+                                  entries or 32 open MARKs in one blob (the pass's 28.1 KiB per-task scratch).          */
 
 #define B9_TF_TASK_MSG  0x08u  /* the payload is a TaskMessage record as TaskQueuePop returns it (pkg/abstractions/taskqueue/taskqueue.go:
                                   238-309): the JSON TaskMessage.Encode writes (pkg/types/task.go:79-90) — a popped record, or the one
@@ -285,6 +303,10 @@ int64_t  b9_drain(b9_ctx *ctx, int handler, uint32_t max_tasks, b9_results *out)
  * pipelines drains (launch k+1 while it post-processes k) keeps the GPU busy back to back this way. */
 #define B9_DRAIN_PEEK  1
 #define B9_DRAIN_ASYNC 2
+/* B9_DRAIN_PICKLE_FULL: B9_TF_PICKLE tasks beyond identity's one-str shape (see B9_TF_PICKLE). Opt-in: without it every
+ * drain answers as before. b9_drain_launch ignores flag bits it does not know, so a library older than this flag answers
+ * these tasks B9_ST_UNSUPPORTED as before, which is never a wrong answer. */
+#define B9_DRAIN_PICKLE_FULL 4
 int64_t  b9_drain_launch(b9_ctx *ctx, int handler, uint32_t max_tasks, int flags);
 int64_t  b9_drain_fetch(b9_ctx *ctx, b9_results *out);
 
