@@ -84,6 +84,7 @@ SYMBOLS = {
     "b9_drain": (C.c_int64, [C.c_void_p, C.c_int, C.c_uint32, C.POINTER(Results)]),
     "b9_drain_launch": (C.c_int64, [C.c_void_p, C.c_int, C.c_uint32, C.c_int]),
     "b9_drain_fetch": (C.c_int64, [C.c_void_p, C.POINTER(Results)]),
+    "b9_endpoint_drain_launch": (C.c_int64, [C.c_void_p, C.c_int, C.c_uint32, C.c_int]),
     "b9_wire_encode": (C.c_int64, [C.c_void_p, C.POINTER(WireEnv), C.c_uint32]),
     "b9_wire_encode_full": (C.c_int64, [C.c_void_p, C.POINTER(WireEnv), C.c_uint32]),
     "b9_comm_unique_id": (C.c_int, [C.c_void_p]),

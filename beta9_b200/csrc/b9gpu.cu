@@ -41,6 +41,10 @@
 cudaError_t launch_wire_encode_full(const void* args, size_t args_size, const void* env, uint32_t grid, cudaStream_t s);
 // pickle_pass_kernel for B9_DRAIN_PICKLE_FULL, from function_drain.cu; args: the drain's DrainArgs
 cudaError_t launch_pickle_pass(const void* args, size_t args_size, int handler, int sm_count, cudaStream_t s);
+// endpoint_drain_kernel for b9_endpoint_drain_launch, from endpoint_drain.cu; args: the drain's DrainArgs, with tile_tasks
+// = ENDPOINT_TILE_TASKS and n_tiles set for it
+cudaError_t launch_endpoint_drain(const void* args, size_t args_size, int handler, int sm_count, cudaStream_t s);
+constexpr uint32_t ENDPOINT_TILE_TASKS = 32;   // endpoint_drain.cu's EP_TILE (the launcher refuses any other)
 
 using namespace b9;
 
@@ -889,9 +893,10 @@ static int finish_launch(b9_ctx* c) {
     return B9_OK;
 }
 
-int64_t b9_drain_launch(b9_ctx* c, int handler, uint32_t max_tasks, int peek) {
-    if (!c) return fail(B9_EINVAL, "b9_drain_launch: ctx is NULL");
-    if (handler < 0 || handler >= B9_H_COUNT_) return fail(B9_ENOSYS, "b9_drain_launch: unknown handler %d", handler);
+// What b9_drain_launch and b9_endpoint_drain_launch share: the window snapshot, the segment waits, the epoch and the
+// control ring, the count-mode prefixes, the stats and the finish. endpoint: answer with endpoint_drain_kernel (the
+// endpoint runner's responses) instead of drain3_kernel (the task-queue runner's results).
+static int64_t drain_launch_common(b9_ctx* c, int handler, uint32_t max_tasks, int peek, bool endpoint) {
     std::lock_guard<std::mutex> out_lk(c->out_mu);
     CU(cudaSetDevice(c->device));
     // results of an earlier launch that were never fetched are dropped; their tasks are still
@@ -966,19 +971,38 @@ int64_t b9_drain_launch(b9_ctx* c, int handler, uint32_t max_tasks, int peek) {
     c->last_op_drain = false;
     cudaError_t le;
     uint32_t tt = 0;
-    switch (handler) {
+    if (endpoint) {
+        // never a programmatic dependent, and the next drain3_kernel is not launched as its dependent either: the timed
+        // span ends right behind it (end_drain_span below), which leaves last_op_drain false. The kernel zeroes the next
+        // control block itself, as drain3_kernel does (endpoint_drain.cu).
+        a.tile_tasks = ENDPOINT_TILE_TASKS;
+        a.n_tiles = (n + ENDPOINT_TILE_TASKS - 1) / ENDPOINT_TILE_TASKS;
+        if (a.count_mode) {                                                 // record indices: ready tasks before each tile
+            const uint32_t blocks = (n + TC_SLOTS - 1u) / TC_SLOTS;
+            tile_count_kernel<<<blocks, TC_SLOTS, 0, s>>>(a.hdr, a.slot_mask, a.first_task, n, ENDPOINT_TILE_TASKS, (uint32_t*)a.tile_base, (uint32_t*)a.block_base);
+            tile_scan_kernel<<<1, 1024, 0, s>>>((uint32_t*)a.block_base, blocks);
+            le = cudaGetLastError();
+        } else le = cudaSuccess;
+        if (le == cudaSuccess) le = launch_endpoint_drain(&a, sizeof a, handler, c->sm_count, s);
+        if (le != cudaSuccess) { c->ctl_dirty = true; return fail(B9_EIO, "endpoint drain kernel launch failed: %s", cudaGetErrorString(le)); }
+        c->last_op_drain = true;
+        c->burst_open = true;
+        end_drain_span(c);
+    } else switch (handler) {
     case B9_H_IDENTITY: le = launch_drain3<0>(a, in_bytes / n, win_max_len, c->stage_bytes_override, c->sm_count, overlap, s, &grid, &tt); break;
     case B9_H_CRC32:    le = launch_drain3<1>(a, in_bytes / n, win_max_len, c->stage_bytes_override, c->sm_count, overlap, s, &grid, &tt); break;
     case B9_H_VADD_F32: le = launch_drain3<2>(a, in_bytes / n, win_max_len, c->stage_bytes_override, c->sm_count, overlap, s, &grid, &tt); break;
     default:            le = launch_drain3<3>(a, in_bytes / n, win_max_len, c->stage_bytes_override, c->sm_count, overlap, s, &grid, &tt); break;
     }
-    if (le != cudaSuccess) { c->ctl_dirty = true; return fail(B9_EIO, "drain kernel launch failed: %s", cudaGetErrorString(le)); }
-    c->last_op_drain = true;
-    c->burst_open = true;
+    if (!endpoint) {
+        if (le != cudaSuccess) { c->ctl_dirty = true; return fail(B9_EIO, "drain kernel launch failed: %s", cudaGetErrorString(le)); }
+        c->last_op_drain = true;
+        c->burst_open = true;
+    }
     // the function path beyond identity's one-str template: a pass over the window's pickle tasks that rewrites the records
     // drain3_kernel left UNSUPPORTED. The next drain kernel waits for it in full (no programmatic dependent launch), and
     // the timed span ends behind it.
-    const bool pickle_pass = (peek & B9_DRAIN_PICKLE_FULL) && win_pickle;
+    const bool pickle_pass = !endpoint && (peek & B9_DRAIN_PICKLE_FULL) && win_pickle;
     if (pickle_pass) {
         a.tile_tasks = tt;
         le = launch_pickle_pass(&a, sizeof a, handler, c->sm_count, s);
@@ -996,6 +1020,19 @@ int64_t b9_drain_launch(b9_ctx* c, int handler, uint32_t max_tasks, int peek) {
     if (peek & B9_DRAIN_ASYNC) return (int64_t)n;   // records = n minus the cancelled slots: known after b9_sync / b9_drain_fetch
     int rc = finish_launch(c);
     return rc ? rc : (int64_t)c->res_n;
+}
+
+int64_t b9_drain_launch(b9_ctx* c, int handler, uint32_t max_tasks, int peek) {
+    if (!c) return fail(B9_EINVAL, "b9_drain_launch: ctx is NULL");
+    if (handler < 0 || handler >= B9_H_COUNT_) return fail(B9_ENOSYS, "b9_drain_launch: unknown handler %d", handler);
+    return drain_launch_common(c, handler, max_tasks, peek, false);
+}
+
+int64_t b9_endpoint_drain_launch(b9_ctx* c, int handler, uint32_t max_tasks, int flags) {
+    if (!c) return fail(B9_EINVAL, "b9_endpoint_drain_launch: ctx is NULL");
+    if (handler < 0 || handler >= B9_H_COUNT_) return fail(B9_ENOSYS, "b9_endpoint_drain_launch: unknown handler %d", handler);
+    if (flags & ~(B9_DRAIN_PEEK | B9_DRAIN_ASYNC)) return fail(B9_EINVAL, "b9_endpoint_drain_launch: unknown flag bits 0x%x", flags);
+    return drain_launch_common(c, handler, max_tasks, flags, true);
 }
 
 int64_t b9_drain_fetch(b9_ctx* c, b9_results* out) {

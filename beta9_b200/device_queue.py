@@ -172,16 +172,25 @@ class DeviceQueue:
         return marked, outcome[:n]
 
     # ---- consumer side
-    def drain(self, handler: str, max_tasks: int = 1 << 22, cap_bytes: Optional[int] = None, full_pickle: bool = False) -> DrainResult:
-        """full_pickle=True (B9_DRAIN_PICKLE_FULL): pickle-framed tasks of every handler over plain values (include/b9gpu.h)."""
-        h = HANDLERS[handler]
-        n = self._check(self._lib.b9_drain_launch(self._ctx, h, max_tasks, L.DRAIN_PICKLE_FULL if full_pickle else 0))
+    def drain(self, handler: str, max_tasks: int = 1 << 22, cap_bytes: Optional[int] = None, full_pickle: bool = False,
+              endpoint: bool = False) -> DrainResult:
+        """full_pickle=True (B9_DRAIN_PICKLE_FULL): pickle-framed tasks of every handler over plain values (include/b9gpu.h).
+        endpoint=True (b9_endpoint_drain_launch): B9_TF_HTTP_BODY tasks answered with the endpoint runner's response bodies."""
+        n = self._launch(HANDLERS[handler], max_tasks, L.DRAIN_PICKLE_FULL if full_pickle else 0, endpoint)
         return self._fetch(n, cap_bytes)
 
-    def drain_launch(self, handler: str, max_tasks: int = 1 << 22, peek: bool = False, wait: bool = True, full_pickle: bool = False) -> int:
+    def drain_launch(self, handler: str, max_tasks: int = 1 << 22, peek: bool = False, wait: bool = True, full_pickle: bool = False,
+                     endpoint: bool = False) -> int:
         """wait=False (B9_DRAIN_ASYNC): returns once the kernels are enqueued; `sync()` or `fetch()` completes it."""
         flags = (1 if peek else 0) | (0 if wait else 2) | (L.DRAIN_PICKLE_FULL if full_pickle else 0)
-        return self._check(self._lib.b9_drain_launch(self._ctx, HANDLERS[handler], max_tasks, flags))
+        return self._launch(HANDLERS[handler], max_tasks, flags, endpoint)
+
+    def _launch(self, h: int, max_tasks: int, flags: int, endpoint: bool) -> int:
+        if not endpoint:
+            return self._check(self._lib.b9_drain_launch(self._ctx, h, max_tasks, flags))
+        if flags & L.DRAIN_PICKLE_FULL:
+            raise ValueError("endpoint=True answers HTTP bodies only: it does not combine with full_pickle=True")
+        return self._check(self._lib.b9_endpoint_drain_launch(self._ctx, h, max_tasks, flags))
 
     def fetch(self, cap_bytes: Optional[int] = None) -> DrainResult:
         self.sync()                                  # completes a wait=False launch: its byte count sizes the buffers below
@@ -205,9 +214,9 @@ class DeviceQueue:
         got = self._check(self._lib.b9_drain_fetch(self._ctx, C.byref(r)))
         return DrainResult(ids[:got], status[:got], has[:got], off[:got], ln[:got], pl[:int(r.n_bytes)], int(r.n_popped), float(r.task_duration))
 
-    def drain_object(self, handler: str, max_tasks: int = 1 << 22) -> np.ndarray:
+    def drain_object(self, handler: str, max_tasks: int = 1 << 22, endpoint: bool = False) -> np.ndarray:
         """One drain whose records land as ONE result-sink object (b9_drain_fetch_object): header + index + blob."""
-        self._check(self._lib.b9_drain_launch(self._ctx, HANDLERS[handler], max_tasks, 0))
+        self._launch(HANDLERS[handler], max_tasks, 0, endpoint)
         need = C.c_uint64(0)
         probe = np.zeros(128, np.uint8)
         rc = self._lib.b9_drain_fetch_object(self._ctx, probe.ctypes.data, 0, C.byref(need))      # B9_ENOSPC: tells the size, consumes nothing

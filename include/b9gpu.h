@@ -310,6 +310,28 @@ int64_t  b9_drain(b9_ctx *ctx, int handler, uint32_t max_tasks, b9_results *out)
 int64_t  b9_drain_launch(b9_ctx *ctx, int handler, uint32_t max_tasks, int flags);
 int64_t  b9_drain_fetch(b9_ctx *ctx, b9_results *out);
 
+/* b9_endpoint_drain_launch: the same window, pop / claim, b9_running, B9_DRAIN_PEEK, B9_DRAIN_ASYNC, return value,
+ * B9_ENOSPC and task_duration as b9_drain_launch (records fetched with b9_drain_fetch or b9_drain_fetch_object), but
+ * every record is what a non-ASGI `@endpoint` answers its caller: the gateway's SerializeHttpPayload and
+ * json.Marshal(TaskPayload) (pkg/abstractions/endpoint/buffer.go:460-572), the runner's json.loads, args / kwargs None
+ * -> [] / {}, handler(*args, **kwargs) and JSONResponse(result) (sdk/src/beta9/runner/endpoint.py:202-306). Per task:
+ *   B9_ST_COMPLETE, has_result = 1   200: the bytes are exactly JSONResponse(result).body -- json.dumps with
+ *                                    ensure_ascii=False and separators "," ":" -- falsy results included
+ *                                    ("" -> "", 0 -> 0, [] -> [], crc32 of "" -> 0)
+ *   B9_ST_REJECTED                   SerializeHttpPayload failed: the gateway answers 400 {"error":"invalid request payload"}
+ *   B9_ST_ERROR                      the handler raised: the runner answers 500 with its traceback, which the host composes
+ *   B9_ST_UNSUPPORTED                not answered on the device; the host runs the reference's path:
+ *                                      a task whose flags are not exactly B9_TF_HTTP_BODY (pre-marshalled payloads,
+ *                                      B9_TF_PICKLE, B9_TF_TASK_MSG);
+ *                                      a render failure (json_sum's total is +-inf or NaN: allow_nan=False raises and the
+ *                                      runner answers 500 with the task Complete);
+ *                                      what the HTTP-body parse and the handlers decline: more than 19 significant digits
+ *                                      at a rounding boundary, nesting deeper than 16, more than 64 members, json_sum ints
+ *                                      outside a C long, vadd_f32 base64 written with escapes.
+ * `flags`: B9_DRAIN_PEEK and B9_DRAIN_ASYNC; any other bit is B9_EINVAL. A separate symbol rather than a b9_drain_launch
+ * flag, because older libraries ignore unknown flag bits and would answer with task-queue bytes; probe it with dlsym. */
+int64_t  b9_endpoint_drain_launch(b9_ctx *ctx, int handler, uint32_t max_tasks, int flags);
+
 /* ---- queue wire records ------------------------------------------------------------------------
  * b9_wire_encode materialises, for the first max_tasks pending tasks (they stay pending), the bytes
  * `TaskMessage.Encode` produces (pkg/types/task.go:55-65,79-90) — what client.Push RPUSHes
