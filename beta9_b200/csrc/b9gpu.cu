@@ -230,6 +230,23 @@ bool place_segment(b9_ctx* c, uint64_t bytes, uint64_t* start) {
     return b9_ring_place(c->ring_bytes, !c->segs.empty(), c->segs.empty() ? 0 : c->segs.front().phys_start, c->write_pos, live, bytes, start) != 0;
 }
 
+// the context's result staging, with `ctl` as the control block whose byte cursor places the records' bytes
+DrainOut drain_out(const b9_ctx* c, DrainCtl* ctl) {
+    DrainOut o;
+    o.payload = c->d_out_payload; o.cap = c->max_result_bytes; o.off = c->d_out_off; o.len = c->d_out_len;
+    o.ids = c->d_out_ids; o.status = c->d_out_status; o.has = c->d_out_has; o.ctl = ctl;
+    return o;
+}
+
+// count mode (cancelled slots in the window): the ready-count prefix per warp-tile of `tile_tasks` slots that gives every
+// record its index (tile_count_kernel + tile_scan_kernel, read by tile_ready_before)
+cudaError_t launch_tile_counts(const DrainArgs& a, uint32_t tile_tasks, cudaStream_t s) {
+    const uint32_t blocks = (a.n_tasks + TC_SLOTS - 1u) / TC_SLOTS;
+    tile_count_kernel<<<blocks, TC_SLOTS, 0, s>>>(a.hdr, a.slot_mask, a.first_task, a.n_tasks, tile_tasks, (uint32_t*)a.tile_base, (uint32_t*)a.block_base);
+    tile_scan_kernel<<<1, 1024, 0, s>>>((uint32_t*)a.block_base, blocks);
+    return cudaGetLastError();
+}
+
 // every warp owns a slice of dynamic shared memory = control block + one stage buffer.
 template <int H> uint32_t drain3_warp_stride(uint32_t in_cap) {
     const size_t ctl = (sizeof(D3Warp<D3Cfg<H>::T>) + 127u) & ~(size_t)127u;
@@ -287,11 +304,8 @@ template <int H> cudaError_t launch_drain3(DrainArgs a, uint64_t avg_task_bytes,
     // switch made vadd_f32 slower, so it stays on pure work stealing like crc32 / json_sum.
     // B9_STATIC_ROUNDS=0 turns it off.
     static const bool allow_static = !(getenv("B9_STATIC_ROUNDS") && atoi(getenv("B9_STATIC_ROUNDS")) == 0);
-    if (a.count_mode) {                                                    // cancelled slots in the window: ready-count prefix per warp-tile
-        const uint32_t blocks = (a.n_tasks + TC_SLOTS - 1u) / TC_SLOTS;
-        tile_count_kernel<<<blocks, TC_SLOTS, 0, s>>>(a.hdr, a.slot_mask, a.first_task, a.n_tasks, tt, (uint32_t*)a.tile_base, (uint32_t*)a.block_base);
-        tile_scan_kernel<<<1, 1024, 0, s>>>((uint32_t*)a.block_base, blocks);
-        e = cudaGetLastError();
+    if (a.count_mode) {
+        e = launch_tile_counts(a, tt, s);
         if (e != cudaSuccess) return e;
     }
     if (allow_static && H == B9_H_IDENTITY) {
@@ -313,6 +327,35 @@ template <int H> cudaError_t launch_drain3(DrainArgs a, uint64_t avg_task_bytes,
     e = cudaLaunchKernelEx(&cfg, drain3_kernel<H>, a, in_cap, stride);
     if (e != cudaSuccess) return e;
     return cudaGetLastError();
+}
+
+// Turns a pushed batch's relative offsets into ring slots (off, hdr, cold metadata).
+__global__ void ingest_kernel(const uint64_t* __restrict__ rel_off, uint32_t n, uint64_t seg_start, uint64_t first_task, uint32_t slot_mask,
+                              const int64_t* __restrict__ ts, const int64_t* __restrict__ exp, const uint8_t* __restrict__ retries,
+                              const uint8_t* __restrict__ flags, uint64_t* __restrict__ off, uint64_t* __restrict__ hdr,
+                              int64_t* __restrict__ ring_ts, int64_t* __restrict__ ring_exp) {
+    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    uint32_t slot = (uint32_t)((first_task + i) & slot_mask);
+    uint64_t o0 = rel_off[0], o = rel_off[i], o1 = rel_off[i + 1];
+    off[slot] = seg_start + (o - o0);
+    hdr[slot] = hdr_pack((uint32_t)(o1 - o), flags ? flags[i] : 0, retries ? retries[i] : 0);
+    ring_ts[slot] = ts ? ts[i] : 0;
+    ring_exp[slot] = exp ? exp[i] : 0;
+}
+
+// Marks expired pending tasks as cancelled (Dispatcher.monitor's unclaimed branch, dispatch.go:173-230).
+__global__ void expire_kernel(uint64_t* __restrict__ hdr, const int64_t* __restrict__ expires, uint32_t slot_mask,
+                              uint64_t first_task, uint32_t n, int64_t now_ns, unsigned long long* __restrict__ count) {
+    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    uint32_t slot = (uint32_t)((first_task + i) & slot_mask);
+    int64_t e = expires[slot];
+    uint64_t h = hdr[slot];
+    if (e != 0 && e <= now_ns && !(hdr_flags(h) & 1u)) {
+        hdr[slot] = h | (1ull << 32);
+        atomicAdd(count, 1ull);
+    }
 }
 
 __global__ void count_cancelled_kernel(const uint64_t* __restrict__ hdr, uint32_t slot_mask, uint64_t first_task, uint32_t n, unsigned long long* __restrict__ count) {
@@ -942,8 +985,7 @@ static int64_t drain_launch_common(b9_ctx* c, int handler, uint32_t max_tasks, i
     DrainArgs a{};
     a.payload = c->d_payload; a.off = c->d_off; a.hdr = c->d_hdr; a.ids = c->d_ids; a.slot_mask = c->slot_mask;
     a.first_task = head; a.n_tasks = n; a.n_tiles = 0;                     // (set per handler by launch_drain3)
-    a.out_payload = c->d_out_payload; a.out_cap = c->max_result_bytes; a.out_off = c->d_out_off; a.out_ids = c->d_out_ids;
-    a.out_status = c->d_out_status; a.out_has = c->d_out_has; a.out_len = c->d_out_len; a.tile_base = (const uint32_t*)c->d_tile_state; a.block_base = (const uint32_t*)c->d_tile_state + ((size_t)c->max_drain_tasks / D2_THREADS + 2); a.handler = handler;
+    a.tile_base = (const uint32_t*)c->d_tile_state; a.block_base = (const uint32_t*)c->d_tile_state + ((size_t)c->max_drain_tasks / D2_THREADS + 2);
     a.count_mode = count_mode;
     a.slow = c->d_slow; a.crc_shift_tabs = c->d_crc_shift;
     a.static_rounds = 0;
@@ -957,7 +999,7 @@ static int64_t drain_launch_common(b9_ctx* c, int handler, uint32_t max_tasks, i
     // the control block: the previous drain kernel zeroed this one (drain_kernel.cuh, D3_CTL_RING), unless something
     // else ran since that the host cannot see through (a failed launch, the wire encoder, the epoch's wrap)
     c->ctl_last = a.epoch % D3_CTL_RING;
-    a.ctl = c->d_ctl + c->ctl_last; a.ctl_next = c->d_ctl + (a.epoch + 1u) % D3_CTL_RING;
+    a.out = drain_out(c, c->d_ctl + c->ctl_last); a.ctl_next = c->d_ctl + (a.epoch + 1u) % D3_CTL_RING;
     if (c->ctl_dirty) {
         c->last_op_drain = false;
         CU(cudaMemsetAsync(c->d_ctl, 0, D3_CTL_RING * sizeof(DrainCtl), s));
@@ -977,12 +1019,7 @@ static int64_t drain_launch_common(b9_ctx* c, int handler, uint32_t max_tasks, i
         // control block itself, as drain3_kernel does (endpoint_drain.cu).
         a.tile_tasks = ENDPOINT_TILE_TASKS;
         a.n_tiles = (n + ENDPOINT_TILE_TASKS - 1) / ENDPOINT_TILE_TASKS;
-        if (a.count_mode) {                                                 // record indices: ready tasks before each tile
-            const uint32_t blocks = (n + TC_SLOTS - 1u) / TC_SLOTS;
-            tile_count_kernel<<<blocks, TC_SLOTS, 0, s>>>(a.hdr, a.slot_mask, a.first_task, n, ENDPOINT_TILE_TASKS, (uint32_t*)a.tile_base, (uint32_t*)a.block_base);
-            tile_scan_kernel<<<1, 1024, 0, s>>>((uint32_t*)a.block_base, blocks);
-            le = cudaGetLastError();
-        } else le = cudaSuccess;
+        le = a.count_mode ? launch_tile_counts(a, ENDPOINT_TILE_TASKS, s) : cudaSuccess;
         if (le == cudaSuccess) le = launch_endpoint_drain(&a, sizeof a, handler, c->sm_count, s);
         if (le != cudaSuccess) { c->ctl_dirty = true; return fail(B9_EIO, "endpoint drain kernel launch failed: %s", cudaGetErrorString(le)); }
         c->last_op_drain = true;
@@ -1157,8 +1194,7 @@ static int64_t wire_encode(b9_ctx* c, const b9_wire_env* env, uint32_t max_tasks
     WireArgs a{};
     a.payload = c->d_payload; a.off = c->d_off; a.hdr = c->d_hdr; a.ids = c->d_ids; a.ts = c->d_ts; a.exp = c->d_exp;
     a.slot_mask = c->slot_mask; a.first_task = head; a.n_tasks = n;
-    a.out_payload = c->d_out_payload; a.out_cap = c->max_result_bytes; a.out_off = c->d_out_off; a.out_len = c->d_out_len;
-    a.out_ids = c->d_out_ids; a.out_status = c->d_out_status; a.out_has = c->d_out_has; a.ctl = c->d_ctl;
+    a.out = drain_out(c, c->d_ctl);
     CU(cudaEventRecord(c->ev_a, s));
     if (full) CU(launch_wire_encode_full(&a, sizeof a, c->d_wire_env, (n + 127) / 128, s));
     else wire_encode_kernel<false><<<(n + 127) / 128, 128, 0, s>>>(a, c->d_wire_env);

@@ -179,17 +179,19 @@ __device__ __forceinline__ void group_copy(uint8_t* __restrict__ dst, const uint
 // ------------------------------------------------------------------ chunk-parallel string transcoding
 // body = the bytes between the frame's quotes. A "unit" is what Go's unquote consumes at once: a
 // plain byte, an escape, a \uXXXX (with its low surrogate partner), a UTF-8 sequence.
-// four hex digits -> their value, or -1; all four bytes at once (no per-digit branch: the callers sit in
-// code that runs one lane per escape)
-__device__ __forceinline__ int hex4(const uint8_t* __restrict__ b) {
-    const uint32_t w = (uint32_t)b[0] | ((uint32_t)b[1] << 8) | ((uint32_t)b[2] << 16) | ((uint32_t)b[3] << 24);
+// four hex digits given as a little-endian word -> their value, or -1; all four at once (no per-digit branch: the
+// callers sit in code that runs one lane per escape)
+__device__ __forceinline__ int hex4w(uint32_t w) {
     const uint32_t H = 0x80808080u;
     const uint32_t x = w & 0x7F7F7F7Fu, y = x | 0x20202020u;
     const uint32_t isd = ((x + 0x50505050u) & ~(x + 0x46464646u)) & H;    // '0' <= x <= '9'
     const uint32_t isl = ((y + 0x1F1F1F1Fu) & ~(y + 0x19191919u)) & H;    // 'a' <= (x | 0x20) <= 'f'
-    if ((isd | isl) != H || (w & H)) return -1;
     const uint32_t nib = (x & 0x0F0F0F0Fu) + (isl >> 7) * 9u;
-    return (int)(((nib & 0xFu) << 12) | (((nib >> 8) & 0xFu) << 8) | (((nib >> 16) & 0xFu) << 4) | (nib >> 24));
+    const int v = (int)(((nib & 0xFu) << 12) | (((nib >> 8) & 0xFu) << 8) | (((nib >> 16) & 0xFu) << 4) | (nib >> 24));
+    return ((isd | isl) != H || (w & H)) ? -1 : v;
+}
+__device__ __forceinline__ int hex4(const uint8_t* __restrict__ b) {
+    return hex4w((uint32_t)b[0] | ((uint32_t)b[1] << 8) | ((uint32_t)b[2] << 16) | ((uint32_t)b[3] << 24));
 }
 __device__ __forceinline__ uint32_t bs_run_before(const uint8_t* __restrict__ b, uint32_t q) {   // backslashes ending at q-1
     uint32_t r = 0;
@@ -306,12 +308,6 @@ __device__ __forceinline__ uint32_t warp_sum(uint32_t v) {
     #pragma unroll
     for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(0xffffffffu, v, d);
     return v;
-}
-__device__ __forceinline__ uint32_t warp_excl_scan(uint32_t v, int lane) {
-    uint32_t inc = v;
-    #pragma unroll
-    for (int d = 1; d < 32; d <<= 1) { uint32_t t = __shfl_up_sync(0xffffffffu, inc, d); if (lane >= d) inc += t; }
-    return inc - v;
 }
 
 __device__ __forceinline__ bool plain_byte(uint32_t c) { return c >= 0x20u && c < 0x7Fu && c != '"' && c != '\\'; }
@@ -557,7 +553,6 @@ __device__ __forceinline__ uint8_t json_cls_of(uint32_t c) {
     }
 }
 __device__ __forceinline__ uint32_t prefix_xor32(uint32_t x) { x ^= x << 1; x ^= x << 2; x ^= x << 4; x ^= x << 8; x ^= x << 16; return x; }
-__device__ __forceinline__ uint32_t lane_prev(uint32_t m, int lane) { const uint32_t v = __shfl_up_sync(0xffffffffu, m, 1); return lane ? v : 0u; }
 // the mask of the lane below; lane 0 gets `carry` (the last lane's mask of the previous segment). Every lane executes the shuffle.
 __device__ __forceinline__ uint32_t lane_prev_carry(uint32_t m, int lane, uint32_t carry) { const uint32_t v = __shfl_up_sync(0xffffffffu, m, 1); return lane ? v : carry; }
 // parity of `bit` over the lanes below this one
@@ -859,17 +854,10 @@ __global__ void __launch_bounds__(1024) tile_scan_kernel(uint32_t* __restrict__ 
     const uint32_t lo = min(blocks, tid * per), hi = min(blocks, lo + per);
     uint32_t sum = 0;
     for (uint32_t i = lo; i < hi; ++i) sum += block_tot[i + 1u];
-    uint32_t inc = sum;
-    #pragma unroll
-    for (int d = 1; d < 32; d <<= 1) { const uint32_t v = __shfl_up_sync(0xffffffffu, inc, d); if ((int)lane >= d) inc += v; }
+    const uint32_t inc = warp_incl_scan(sum, (int)lane);
     if (lane == 31) s_warp[warp] = inc;
     __syncthreads();
-    if (warp == 0) {
-        uint32_t x = s_warp[lane], y = x;
-        #pragma unroll
-        for (int d = 1; d < 32; d <<= 1) { const uint32_t v = __shfl_up_sync(0xffffffffu, y, d); if ((int)lane >= d) y += v; }
-        s_warp[lane] = y - x;                                             // exclusive over warps
-    }
+    if (warp == 0) s_warp[lane] = warp_excl_scan(s_warp[lane], (int)lane);   // exclusive over warps
     __syncthreads();
     uint32_t run = s_warp[warp] + inc - sum;                              // ready tasks before my first block
     for (uint32_t i = lo; i < hi; ++i) { run += block_tot[i + 1u]; block_tot[i + 1u] = run; }
@@ -1033,17 +1021,6 @@ __device__ __forceinline__ uint32_t esc16(uint32_t bs, uint32_t cin, uint32_t cn
     *cout = cnt < 16u ? (escaped >> cnt) & 1u : (seq_even >> 16) & 1u;
     return escaped;
 }
-// four hex digits given as a little-endian word -> their value, or -1 (SWAR, no loads)
-__device__ __forceinline__ int hex4w(uint32_t w) {
-    const uint32_t H = 0x80808080u;
-    const uint32_t x = w & 0x7F7F7F7Fu, y = x | 0x20202020u;
-    const uint32_t isd = ((x + 0x50505050u) & ~(x + 0x46464646u)) & H;    // '0' <= x <= '9'
-    const uint32_t isl = ((y + 0x1F1F1F1Fu) & ~(y + 0x19191919u)) & H;    // 'a' <= (x | 0x20) <= 'f'
-    const uint32_t nib = (x & 0x0F0F0F0Fu) + (isl >> 7) * 9u;
-    const int v = (int)(((nib & 0xFu) << 12) | (((nib >> 8) & 0xFu) << 8) | (((nib >> 16) & 0xFu) << 4) | (nib >> 24));
-    return ((isd | isl) != H || (w & H)) ? -1 : v;
-}
-
 // All 32 lanes; the body is sbuf[at, at + n) (stage buffer), `list` is scratch for 256 16-bit positions. true:
 // json.dumps(identity(body)) is the body text as it now stands in the stage buffer (lone surrogates rewritten). false:
 // not decided. The escape starts of a pass are first compacted into `list` (prefix sum over the lanes' counts), then
@@ -1300,18 +1277,9 @@ __device__ __noinline__ void slow_task(const DrainArgs& a, uint64_t goff, uint32
                                        uint32_t stage_cap, int lane) {
     const uint32_t len = lenw & 0x3FFFFFFFu;
     const bool http = (lenw & 0x40000000u) != 0;
-    const uint8_t* p = a.payload + goff;
-    if (len + 32u <= stage_cap) {
-        // the walks below are chains of dependent byte loads: run them against shared memory instead of L2/HBM
-        const uint32_t mis = (uint32_t)(goff & 15ull);
-        const uint4* src = (const uint4*)(p - mis);
-        uint4* dst = (uint4*)stage;
-        const uint32_t nv = (mis + len + 15u) >> 4;
-        __syncwarp();
-        for (uint32_t v = lane; v < nv; v += 32) dst[v] = __ldg(src + v);
-        __syncwarp();
-        p = stage + mis;
-    }
+    // the walks below are chains of dependent byte loads: run them against shared memory instead of L2/HBM
+    const uint8_t* p = stage_one_task(a.payload, goff, len, stage, stage_cap, lane);
+    if (!p) p = a.payload + goff;
     TaskRec rec; rec.ready = 1; rec.status = 0; rec.has = 0; rec.mode = OM_NONE; rec.out_len = 0; rec.src_off = 0; rec.src_len = 0; rec.value = 0;
     bool par = false, fast = false;
     EscLane L; L.start = 0; L.out_len = 0; L.npatch = 0; L.ok = true; L.len_change = false;
@@ -1323,18 +1291,13 @@ __device__ __noinline__ void slow_task(const DrainArgs& a, uint64_t goff, uint32
         w = __shfl_sync(0xffffffffu, w, 0);
         const uint32_t hdr = (w >> 24) & 0x7Fu, n = w & 0xFFFFFFu;
         const uint32_t out_len = w ? 11u + hdr + n + 2u : 0u;
-        unsigned long long base = 0;
-        const uint32_t alloc = (out_len + 15u) & ~15u;
-        if (lane == 0 && out_len) base = atomicAdd(&a.ctl->bytes, (unsigned long long)alloc);
-        base = __shfl_sync(0xffffffffu, base, 0);
-        const bool fits = base + alloc <= a.out_cap;
-        if (!fits && lane == 0) a.ctl->overflow = 1u;
-        if (w && fits) {
-            uint8_t* o = a.out_payload + base;
+        const Reservation r = warp_reserve_bytes(a.out, (out_len + 15u) & ~15u, lane);
+        if (w && r.fits) {
+            uint8_t* o = a.out.payload + r.base;
             if (lane == 0) { pickle_result_header(o, hdr + n + 2u); o[11u + hdr + n + 1u] = 0x2E; }
             warp_copy(o + 11, p + 21, hdr + n + 1u, lane);                 // string opcode + bytes + MEMOIZE
         }
-        if (lane == 0) { a.out_off[j] = fits ? base : 0; a.out_len[j] = out_len; a.out_status[j] = w ? 0 : ST_UNSUPPORTED; a.out_has[j] = w ? 1 : 0; }
+        if (lane == 0) store_record(a.out, j, r.fits, r.base, out_len, w ? 0 : ST_UNSUPPORTED, w ? 1 : 0);
         __syncwarp();
         return;
     }
@@ -1347,21 +1310,16 @@ __device__ __noinline__ void slow_task(const DrainArgs& a, uint64_t goff, uint32
     if (!par) {                                                            // the sequential validating parser decides
         if (lane == 0) {
             // a TaskMessage record: its id is the one the main loop wrote to the record (before it published the item)
-            d2_parse_and_size<0>(p, len, rec, nullptr, http, record ? a.out_ids + j : nullptr);
+            d2_parse_and_size<0>(p, len, rec, nullptr, http, record ? a.out.ids + j : nullptr);
         }
         rec.src_off = __shfl_sync(0xffffffffu, rec.src_off, 0); rec.src_len = __shfl_sync(0xffffffffu, rec.src_len, 0);
         rec.out_len = __shfl_sync(0xffffffffu, rec.out_len, 0);
         const uint32_t w = __shfl_sync(0xffffffffu, (uint32_t)rec.status | ((uint32_t)rec.has << 8) | ((uint32_t)rec.mode << 16), 0);
         rec.status = (uint8_t)w; rec.has = (uint8_t)(w >> 8); rec.mode = (uint8_t)(w >> 16);
     }
-    unsigned long long base = 0;
-    const uint32_t alloc = (rec.out_len + 15u) & ~15u;                     // the cursor moves in 16-byte units (the tiles' ranges stay vector-aligned)
-    if (lane == 0 && rec.out_len) base = atomicAdd(&a.ctl->bytes, (unsigned long long)alloc);
-    base = __shfl_sync(0xffffffffu, base, 0);
-    const bool fits = base + alloc <= a.out_cap;
-    if (!fits && lane == 0) a.ctl->overflow = 1u;
-    if (rec.has && fits) {
-        uint8_t* o = a.out_payload + base;
+    const Reservation r = warp_reserve_bytes(a.out, (rec.out_len + 15u) & ~15u, lane);
+    if (rec.has && r.fits) {
+        uint8_t* o = a.out.payload + r.base;
         if (rec.mode == OM_STR_PAR) {
             if (fast) esc_emit_fast(p + FRAME_PRE_LEN - 1, nbody + 2, lane, o, L);
             else      esc_emit_general(p + FRAME_PRE_LEN, nbody, lane, o, L);
@@ -1369,29 +1327,29 @@ __device__ __noinline__ void slow_task(const DrainArgs& a, uint64_t goff, uint32
         else if (rec.mode == OM_COPY) warp_copy(o, p + rec.src_off, rec.src_len, lane);
         else if (lane == 0) seq_emit<true>(p, rec, o);
     }
-    if (lane == 0) { a.out_off[j] = fits ? base : 0; a.out_len[j] = rec.out_len; a.out_status[j] = rec.status; a.out_has[j] = rec.has; }
+    if (lane == 0) store_record(a.out, j, r.fits, r.base, rec.out_len, rec.status, rec.has);
     __syncwarp();
 }
 
 __device__ __noinline__ void d3_identity_tail(const DrainArgs& a, uint8_t* __restrict__ stage, uint32_t stage_cap, int lane, uint32_t n_workers) {
     __syncwarp();
-    if (lane == 0) { __threadfence(); atomicAdd(&a.ctl->workers_done, 1u); __threadfence(); }
+    if (lane == 0) { __threadfence(); atomicAdd(&a.out.ctl->workers_done, 1u); __threadfence(); }
     for (;;) {
         uint32_t i = 0xFFFFFFFFu;
         if (lane == 0) {
-            const uint32_t n = *(volatile unsigned int*)&a.ctl->n_slow;
-            uint32_t h = *(volatile unsigned int*)&a.ctl->slow_head;
+            const uint32_t n = *(volatile unsigned int*)&a.out.ctl->n_slow;
+            uint32_t h = *(volatile unsigned int*)&a.out.ctl->slow_head;
             while (h < n) {
-                const uint32_t old = atomicCAS(&a.ctl->slow_head, h, h + 1u);
+                const uint32_t old = atomicCAS(&a.out.ctl->slow_head, h, h + 1u);
                 if (old == h) { i = h; break; }
                 h = old;
             }
-            if (i == 0xFFFFFFFFu && *(volatile unsigned int*)&a.ctl->workers_done == n_workers) {
+            if (i == 0xFFFFFFFFu && *(volatile unsigned int*)&a.out.ctl->workers_done == n_workers) {
                 // everybody has published: the list is final — one more look, so that the last worker leaves nothing behind
-                const uint32_t n2 = *(volatile unsigned int*)&a.ctl->n_slow;
-                h = *(volatile unsigned int*)&a.ctl->slow_head;
+                const uint32_t n2 = *(volatile unsigned int*)&a.out.ctl->n_slow;
+                h = *(volatile unsigned int*)&a.out.ctl->slow_head;
                 while (h < n2) {
-                    const uint32_t old = atomicCAS(&a.ctl->slow_head, h, h + 1u);
+                    const uint32_t old = atomicCAS(&a.out.ctl->slow_head, h, h + 1u);
                     if (old == h) { i = h; break; }
                     h = old;
                 }
@@ -1470,7 +1428,7 @@ __global__ void __launch_bounds__(D3_WARPS * 32, (HANDLER == 1 ? B9_CRC_MINB : H
     auto fetch = [&]() -> unsigned long long {                             // lane 0's value is the tile
         unsigned long long t = 0;
         if (q < a.static_rounds) t = wid + q * n_workers;
-        else if (lane == 0) t = dyn_base + atomicAdd(&a.ctl->ticket, 1ull);
+        else if (lane == 0) t = dyn_base + atomicAdd(&a.out.ctl->ticket, 1ull);
         ++q;
         return t;
     };
@@ -1597,8 +1555,9 @@ __global__ void __launch_bounds__(D3_WARPS * 32, (HANDLER == 1 ? B9_CRC_MINB : H
                     }
                 }
             }
-        } else if (HANDLER == 1) {
-            // crc32: the whole warp works on one task at a time (tasks are long and of very different lengths)
+        } else if (HANDLER == 1 || HANDLER == 3) {
+            // crc32 and json_sum: the whole warp works on one task at a time (tasks are long and of very different lengths)
+            const uint32_t* crc_table = HANDLER == 1 ? s_crc_table : nullptr;
             for (uint32_t kt = 0; kt < nt; ++kt) {
                 if (!((ready_mask_t >> kt) & 1u)) continue;
                 const uint32_t fl = W.flg[kt];
@@ -1606,40 +1565,26 @@ __global__ void __launch_bounds__(D3_WARPS * 32, (HANDLER == 1 ? B9_CRC_MINB : H
                     // the function path (identity only), HTTP bodies (map rules), TaskMessage records: the sequential parser
                     if (lane == (int)kt) {
                         if (fl & B9_TF_PICKLE_BIT) rec.status = ST_UNSUPPORTED;
-                        else d2_parse_and_size<1>(staged ? (const uint8_t*)(sbuf + W.soff[kt]) : a.payload + W.goff[kt], W.len[kt], rec, s_crc_table,
-                                                   (fl & B9_TF_HTTP_BODY_BIT) != 0,
-                                                   (fl & B9_TF_TASK_MSG_BIT) ? a.ids + ((a.first_task + t0 + kt) & a.slot_mask) : nullptr);
+                        else d2_parse_and_size<HANDLER>(staged ? (const uint8_t*)(sbuf + W.soff[kt]) : a.payload + W.goff[kt], W.len[kt], rec, crc_table,
+                                                         (fl & B9_TF_HTTP_BODY_BIT) != 0,
+                                                         (fl & B9_TF_TASK_MSG_BIT) ? a.ids + ((a.first_task + t0 + kt) & a.slot_mask) : nullptr);
                     }
                     continue;
                 }
                 const uint8_t* tp = staged ? (const uint8_t*)(sbuf + W.soff[kt]) : stage_one_task(a.payload, W.goff[kt], W.len[kt], sbuf, in_cap, lane);
-                if (tp) crc_task_coop(tp, true, W.len[kt], lane, lane == (int)kt, s_crc_table, a.crc_shift_tabs, rec);
-                else    crc_task_coop(a.payload + W.goff[kt], false, W.len[kt], lane, lane == (int)kt, s_crc_table, a.crc_shift_tabs, rec);
-            }
-        } else if (HANDLER == 3) {
-            // json_sum: the whole warp parses one document at a time
-            for (uint32_t kt = 0; kt < nt; ++kt) {
-                if (!((ready_mask_t >> kt) & 1u)) continue;
-                const uint32_t fl = W.flg[kt];
-                if (fl & (B9_TF_PICKLE_BIT | B9_TF_HTTP_BODY_BIT | B9_TF_TASK_MSG_BIT)) {
-                    // the function path (identity only), HTTP bodies (map rules), TaskMessage records: the sequential parser
+                if constexpr (HANDLER == 1) {
+                    if (tp) crc_task_coop(tp, true, W.len[kt], lane, lane == (int)kt, s_crc_table, a.crc_shift_tabs, rec);
+                    else    crc_task_coop(a.payload + W.goff[kt], false, W.len[kt], lane, lane == (int)kt, s_crc_table, a.crc_shift_tabs, rec);
+                } else {
+                    int done = 0; unsigned long long sum = 0;
+                    if (tp) {                                              // one 1 KiB segment (configs[4]) or up to four
+                        if (W.len[kt] <= 1024u + JSON_PRE_LEN + JSON_SUF_LEN) done = json_sum_coop<false>(tp, W.len[kt], lane, s_jcls, &sum);
+                        else done = json_sum_coop<true>(tp, W.len[kt], lane, s_jcls, &sum);
+                    }
                     if (lane == (int)kt) {
-                        if (fl & B9_TF_PICKLE_BIT) rec.status = ST_UNSUPPORTED;
-                        else d2_parse_and_size<3>(staged ? (const uint8_t*)(sbuf + W.soff[kt]) : a.payload + W.goff[kt], W.len[kt], rec, nullptr,
-                                                   (fl & B9_TF_HTTP_BODY_BIT) != 0,
-                                                   (fl & B9_TF_TASK_MSG_BIT) ? a.ids + ((a.first_task + t0 + kt) & a.slot_mask) : nullptr);
+                        if (done) { if (sum) { rec.value = (long long)sum; rec.out_len = dec_len_u64(sum); rec.mode = OM_I64_DEC; rec.has = 1; } }
+                        else d2_parse_and_size<3>(tp ? tp : a.payload + W.goff[kt], W.len[kt], rec, nullptr);
                     }
-                    continue;
-                }
-                int done = 0; unsigned long long sum = 0;
-                const uint8_t* tp = staged ? (const uint8_t*)(sbuf + W.soff[kt]) : stage_one_task(a.payload, W.goff[kt], W.len[kt], sbuf, in_cap, lane);
-                if (tp) {                                                  // one 1 KiB segment (configs[4]) or up to four
-                    if (W.len[kt] <= 1024u + JSON_PRE_LEN + JSON_SUF_LEN) done = json_sum_coop<false>(tp, W.len[kt], lane, s_jcls, &sum);
-                    else done = json_sum_coop<true>(tp, W.len[kt], lane, s_jcls, &sum);
-                }
-                if (lane == (int)kt) {
-                    if (done) { if (sum) { rec.value = (long long)sum; rec.out_len = dec_len_u64(sum); rec.mode = OM_I64_DEC; rec.has = 1; } }
-                    else d2_parse_and_size<3>(tp ? tp : a.payload + W.goff[kt], W.len[kt], rec, nullptr);
                 }
             }
         } else if (my_pickle) {
@@ -1664,7 +1609,7 @@ __global__ void __launch_bounds__(D3_WARPS * 32, (HANDLER == 1 ? B9_CRC_MINB : H
             advance();
         }
         const uint32_t base_cnt = a.count_mode ? tile_ready_before(a, tile, TT) : t0;   // (count_mode: from the pre-pass kernels)
-        if (lane == 0 && tile == a.n_tiles - 1) a.ctl->total_cnt = base_cnt + rc;
+        if (lane == 0 && tile == a.n_tiles - 1) a.out.ctl->total_cnt = base_cnt + rc;
 
         // ---------------- compaction (ballot) + sizes (scan) + ONE cursor add per warp-tile -------------
         const uint32_t my_bytes = (sub == 0) ? rec.out_len : 0u;
@@ -1677,18 +1622,15 @@ __global__ void __launch_bounds__(D3_WARPS * 32, (HANDLER == 1 ? B9_CRC_MINB : H
         // (identity only: for vadd_f32, whose kernel is bound by the base64 arithmetic, the warp-wide copy's extra
         // instructions cost more than its coalescing saves: it measured slower)
         constexpr bool COAL = (T == 32 && G == 1 && HANDLER == 0);
-        const uint32_t tb_alloc = COAL ? ((tb + 15u) & ~15u) : tb;
-        unsigned long long base = 0;
-        if (lane == 0 && tb) base = atomicAdd(&a.ctl->bytes, (unsigned long long)tb_alloc);
-        base = __shfl_sync(0xffffffffu, base, 0);
-        const bool fits = base + tb_alloc <= a.out_cap;
-        if (!fits && lane == 0) a.ctl->overflow = 1u;
+        const Reservation res = warp_reserve_bytes(a.out, COAL ? ((tb + 15u) & ~15u) : tb, lane);
+        const unsigned long long base = res.base;
+        const bool fits = res.fits;
         bool coal = false;
         if constexpr (COAL) {
             const uint32_t c_len = (mine && rec.has && rec.mode == OM_COPY) ? rec.src_len : 0u;
             const bool ok_me = rec.out_len == c_len && (c_len == 0u || c_len >= 16u);
             coal = staged && fits && tb != 0u && tb <= D3_COPY_MAX_BYTES && __all_sync(0xffffffffu, ok_me);
-            if (coal) d3_copy_tile(W.ct, sbuf, a.out_payload + base, c_len, ex_bytes0, my_soff + rec.src_off, tb, lane);
+            if (coal) d3_copy_tile(W.ct, sbuf, a.out.payload + base, c_len, ex_bytes0, my_soff + rec.src_off, tb, lane);
         }
 
         // ---------------- phase B: G lanes per task ----------------------------------------------------
@@ -1697,23 +1639,23 @@ __global__ void __launch_bounds__(D3_WARPS * 32, (HANDLER == 1 ? B9_CRC_MINB : H
             if (sub == 0) {
                 const uint32_t slot = (uint32_t)((a.first_task + t0 + k) & a.slot_mask);
                 const uint32_t j = base_cnt + ex_cnt;
-                a.out_ids[j] = (G == 1) ? m_id : __ldg(a.ids + slot);
-                if (HANDLER == 0 && rec.mode == OM_DEFER) {                // the second kernel writes the rest of the record
-                    SlowItem* it = a.slow + atomicAdd(&a.ctl->n_slow, 1u);
+                a.out.ids[j] = (G == 1) ? m_id : __ldg(a.ids + slot);
+                if (HANDLER == 0 && rec.mode == OM_DEFER) {                // the kernel's tail writes the rest of the record
+                    SlowItem* it = a.slow + atomicAdd(&a.out.ctl->n_slow, 1u);
                     it->w1 = (unsigned long long)(my_len | (rec.value == 1 ? 0x80000000u : 0u) | (my_http ? 0x40000000u : 0u)) | ((unsigned long long)j << 32) | (rec.value == 2 ? (1ull << 56) : 0ull)
                            | (rec.value == 3 ? (1ull << 57) : 0ull);
                     __threadfence();
                     *(volatile unsigned long long*)&it->w0 = my_goff | ((unsigned long long)a.epoch << 40);
-                } else { a.out_off[j] = fits ? ob : 0; a.out_len[j] = rec.out_len; a.out_status[j] = rec.status; a.out_has[j] = rec.has; }
+                } else store_record(a.out, j, fits, ob, rec.out_len, rec.status, rec.has);
             }
             if (rec.has && fits) {
                 if (rec.mode == OM_COPY) {
                     if (coal) {}                                            // written by d3_copy_tile
-                    else if (staged) group_copy_staged<G>(a.out_payload + ob, sbuf + my_soff + rec.src_off, rec.src_len, sub);
-                    else             group_copy_generic<G>(a.out_payload + ob, a.payload + my_goff + rec.src_off, rec.src_len, sub);
+                    else if (staged) group_copy_staged<G>(a.out.payload + ob, sbuf + my_soff + rec.src_off, rec.src_len, sub);
+                    else             group_copy_generic<G>(a.out.payload + ob, a.payload + my_goff + rec.src_off, rec.src_len, sub);
                 } else if (sub == 0 && rec.mode != OM_STR_PAR) {
                     const uint8_t* p = (staged && !clobbered) ? (const uint8_t*)(sbuf + my_soff) : a.payload + my_goff;
-                    d2_phase_b_task<HANDLER>(p, rec, a.out_payload + ob);
+                    d2_phase_b_task<HANDLER>(p, rec, a.out.payload + ob);
                 }
             }
         }

@@ -1,5 +1,5 @@
-// Shared definitions of the drain: ring slot words, the control block, the argument block, the SDK's
-// canonical frame, and the two small ring kernels (expire, ingest). The drain itself is drain2.cuh.
+// Shared definitions of the drain: ring slot words, the control block, the result records every drain kernel writes
+// (DrainOut and its helpers), the argument block and the SDK's canonical frame. The drain itself is drain2.cuh.
 // Reference behaviour realised per task:
 //     pop + decode   pkg/abstractions/taskqueue/client.go:43-96, taskqueue.go:213-214
 //     loads + call   sdk/src/beta9/runner/taskqueue.py:196-201,349-361
@@ -48,6 +48,56 @@ struct SlowItem {
                                     // | bit 57 = a TaskMessage record (B9_TF_TASK_MSG)
 };
 
+// The result records of a drain (or a wire encoding): record j is ids[j], status[j], has[j] and the bytes
+// payload[off[j], off[j] + len[j]). Every kernel that writes records places their bytes with reserve_bytes /
+// warp_reserve_bytes and writes the rest with store_record.
+struct DrainOut {
+    uint8_t*  payload; uint64_t cap;
+    uint64_t* off;                  // [n_tasks + 1]  start of each record's bytes
+    uint32_t* len;                  // [n_tasks]      length of each record's bytes
+    uint4*    ids;                  // [n_tasks]
+    uint8_t*  status;               // [n_tasks]
+    uint8_t*  has;                  // [n_tasks]
+    DrainCtl* ctl;                  // the byte cursor and the overflow flag; for a drain, this launch's entry of the control ring
+};
+
+// Result bytes are placed by an atomicAdd on ctl->bytes. A reservation that ends past `cap` sets ctl->overflow (the host
+// then reports B9_ENOSPC and consumes nothing); the records it was for get offset 0 and their bytes are not written.
+// The caller chooses the byte count. drain3_kernel's identity tiles round it up to 16 bytes, because d3_copy_tile writes
+// a tile's range with aligned 16-byte stores. slow_task and the pickle pass, which take bytes from the same cursor, round
+// as well so that an identity drain's cursor stays aligned, and the endpoint kernel rounds as identity's tiles do. The
+// other handlers' tiles and the wire encoder reserve exact byte counts: no d3_copy_tile shares their cursor.
+struct Reservation { unsigned long long base; bool fits; };
+
+// one thread reserves `bytes`
+__device__ __forceinline__ Reservation reserve_bytes(const DrainOut& o, uint32_t bytes) {
+    Reservation r; r.base = 0;
+    if (bytes) r.base = atomicAdd(&o.ctl->bytes, (unsigned long long)bytes);
+    r.fits = r.base + bytes <= o.cap;
+    if (!r.fits) o.ctl->overflow = 1u;
+    return r;
+}
+// the whole warp, `bytes` the same on every lane: lane 0 reserves, every lane gets the reservation
+__device__ __forceinline__ Reservation warp_reserve_bytes(const DrainOut& o, uint32_t bytes, int lane) {
+    Reservation r; r.base = 0;
+    if (lane == 0 && bytes) r.base = atomicAdd(&o.ctl->bytes, (unsigned long long)bytes);
+    r.base = __shfl_sync(0xffffffffu, r.base, 0);
+    r.fits = r.base + bytes <= o.cap;
+    if (!r.fits && lane == 0) o.ctl->overflow = 1u;
+    return r;
+}
+// record j except its id; its bytes are at `off` when their reservation fits
+__device__ __forceinline__ void store_record(const DrainOut& o, uint32_t j, bool fits, unsigned long long off, uint32_t len, uint8_t status, uint8_t has) {
+    o.off[j] = fits ? off : 0; o.len[j] = len; o.status[j] = status; o.has[j] = has;
+}
+
+__device__ __forceinline__ uint32_t warp_incl_scan(uint32_t v, int lane) {
+    #pragma unroll
+    for (int d = 1; d < 32; d <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, v, d); if (lane >= d) v += t; }
+    return v;
+}
+__device__ __forceinline__ uint32_t warp_excl_scan(uint32_t v, int lane) { return warp_incl_scan(v, lane) - v; }
+
 struct DrainArgs {
     // ring (inputs)
     const uint8_t*  payload;        // ring bytes
@@ -58,19 +108,10 @@ struct DrainArgs {
     uint64_t first_task;            // logical index of the window's first task
     uint32_t n_tasks;
     uint32_t n_tiles;
-    // outputs
-    uint8_t*  out_payload; uint64_t out_cap;
-    uint64_t* out_off;              // [n_tasks + 1]  start of each record's bytes
-    uint32_t* out_len;              // [n_tasks]      length of each record's bytes
-    uint4*    out_ids;              // [n_tasks]
-    uint8_t*  out_status;           // [n_tasks]
-    uint8_t*  out_has;              // [n_tasks]
-    // control
-    DrainCtl* ctl;                  // this launch's entry of the control ring: ctl[epoch % D3_CTL_RING]
+    DrainOut out;                   // out.ctl: this launch's entry of the control ring, ctl[epoch % D3_CTL_RING]
     DrainCtl* ctl_next;             // the next launch's entry: zeroed by this launch once the previous one has completed
     const uint32_t* tile_base;     // count_mode: [n_tiles] ready tasks before each warp-tile inside its 256-slot block (tile_count_kernel)
     const uint32_t* block_base;     // count_mode: [n / 256 + 1] ready tasks before each 256-slot block (tile_scan_kernel); last = window total
-    int handler;
     uint32_t count_mode;            // 0 = no pending task is cancelled (record index = task index), 1 = record index from tile_base
     SlowItem* slow;                 // identity: [n_tasks] work list of deferred tasks
     uint32_t epoch;                 // identity: this launch's tag in SlowItem.w0 (1 .. 2^24 - 1)
@@ -84,9 +125,6 @@ constexpr uint32_t TC_SLOTS = 256;             // slots per tile_count_kernel bl
 __device__ __forceinline__ uint32_t tile_ready_before(const DrainArgs& a, unsigned long long tile, uint32_t T) {
     return __ldg(a.tile_base + tile) + __ldg(a.block_base + (uint32_t)((tile * T) / TC_SLOTS));
 }
-
-__device__ __forceinline__ uint64_t ld_volatile_u64(const uint64_t* p) { return *(const volatile uint64_t*)p; }
-__device__ __forceinline__ void st_volatile_u64(uint64_t* p, uint64_t v) { *(volatile uint64_t*)p = v; }
 
 // warp-cooperative byte copy global -> global (arbitrary alignment on both sides).
 // 16-byte stores on the destination, 4-byte loads + funnel shift on the source.
@@ -122,34 +160,5 @@ __device__ inline void warp_copy(uint8_t* __restrict__ dst, const uint8_t* __res
 __device__ __constant__ uint8_t FRAME_PRE[11] = {'{', '"', 'a', 'r', 'g', 's', '"', ':', ' ', '[', '"'};
 __device__ __constant__ uint8_t FRAME_SUF[17] = {'"', ']', ',', ' ', '"', 'k', 'w', 'a', 'r', 'g', 's', '"', ':', ' ', '{', '}', '}'};
 constexpr uint32_t FRAME_PRE_LEN = 11, FRAME_SUF_LEN = 17;
-
-// Marks expired pending tasks as cancelled (Dispatcher.monitor's unclaimed branch, dispatch.go:173-230).
-__global__ void expire_kernel(uint64_t* __restrict__ hdr, const int64_t* __restrict__ expires, uint32_t slot_mask,
-                              uint64_t first_task, uint32_t n, int64_t now_ns, unsigned long long* __restrict__ count) {
-    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    uint32_t slot = (uint32_t)((first_task + i) & slot_mask);
-    int64_t e = expires[slot];
-    uint64_t h = hdr[slot];
-    if (e != 0 && e <= now_ns && !(hdr_flags(h) & 1u)) {
-        hdr[slot] = h | (1ull << 32);
-        atomicAdd(count, 1ull);
-    }
-}
-
-// Turns a pushed batch's relative offsets into ring slots (off, hdr, cold metadata).
-__global__ void ingest_kernel(const uint64_t* __restrict__ rel_off, uint32_t n, uint64_t seg_start, uint64_t first_task, uint32_t slot_mask,
-                              const int64_t* __restrict__ ts, const int64_t* __restrict__ exp, const uint8_t* __restrict__ retries,
-                              const uint8_t* __restrict__ flags, uint64_t* __restrict__ off, uint64_t* __restrict__ hdr,
-                              int64_t* __restrict__ ring_ts, int64_t* __restrict__ ring_exp) {
-    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    uint32_t slot = (uint32_t)((first_task + i) & slot_mask);
-    uint64_t o0 = rel_off[0], o = rel_off[i], o1 = rel_off[i + 1];
-    off[slot] = seg_start + (o - o0);
-    hdr[slot] = hdr_pack((uint32_t)(o1 - o), flags ? flags[i] : 0, retries ? retries[i] : 0);
-    ring_ts[slot] = ts ? ts[i] : 0;
-    ring_exp[slot] = exp ? exp[i] : 0;
-}
 
 }  // namespace b9

@@ -9,8 +9,8 @@
 // Shape: persistent warps take warp-tiles of EP_TILE consecutive slots from the control block's ticket, one task per
 // lane. Each lane reads its slot, parses its body (parse_payload, http = true) and runs phase A; a ballot over the
 // non-cancelled lanes gives the record indices (count mode: plus the ready tasks before the tile, from
-// tile_count_kernel run with EP_TILE), one warp scan of the record lengths and one cursor atomicAdd per tile (rounded up
-// to 16 bytes, as drain3_kernel does) place the bytes. Records that are the argument's token verbatim (identity's
+// tile_count_kernel run with EP_TILE), one warp scan of the record lengths and one warp_reserve_bytes per tile
+// (drain_kernel.cuh, rounded up to 16 bytes as it says) place the bytes. Records that are the argument's token verbatim (identity's
 // common string) are copied by the whole warp, one record after the other; every other record is written by its lane.
 //
 // The control ring (drain_kernel.cuh, D3_CTL_RING): this kernel zeroes the next launch's entry itself, as drain3_kernel
@@ -43,7 +43,7 @@ __global__ void __launch_bounds__(EP_WARPS * 32) endpoint_drain_kernel(b9::Drain
     const int lane = threadIdx.x & 31;
     for (;;) {
         unsigned long long tile = 0;
-        if (lane == 0) tile = atomicAdd(&a.ctl->ticket, 1ull);
+        if (lane == 0) tile = atomicAdd(&a.out.ctl->ticket, 1ull);
         tile = __shfl_sync(0xffffffffu, tile, 0);
         if (tile >= a.n_tiles) break;
         const uint32_t i = (uint32_t)tile * EP_TILE + (uint32_t)lane;
@@ -64,27 +64,20 @@ __global__ void __launch_bounds__(EP_WARPS * 32) endpoint_drain_kernel(b9::Drain
         // ---- record index (ballot), bytes (scan) and ONE cursor add per warp-tile
         const uint32_t live_mask = __ballot_sync(0xffffffffu, live);
         const uint32_t base_cnt = a.count_mode ? b9::tile_ready_before(a, tile, EP_TILE) : (uint32_t)tile * EP_TILE;
-        if (lane == 0 && tile == a.n_tiles - 1) a.ctl->total_cnt = base_cnt + __popc(live_mask);
+        if (lane == 0 && tile == a.n_tiles - 1) a.out.ctl->total_cnt = base_cnt + __popc(live_mask);
         const uint32_t j = base_cnt + __popc(live_mask & ((1u << lane) - 1u));
         const uint32_t my = rec.has ? rec.out_len : 0u;
-        uint32_t incl = my;
-        #pragma unroll
-        for (int d = 1; d < 32; d <<= 1) { const uint32_t v = __shfl_up_sync(0xffffffffu, incl, d); if (lane >= d) incl += v; }
+        const uint32_t incl = b9::warp_incl_scan(my, lane);
         const uint32_t tb = __shfl_sync(0xffffffffu, incl, 31);
-        const uint32_t tb_alloc = (tb + 15u) & ~15u;
-        unsigned long long base = 0;
-        if (lane == 0 && tb) base = atomicAdd(&a.ctl->bytes, (unsigned long long)tb_alloc);
-        base = __shfl_sync(0xffffffffu, base, 0);
-        const bool fits = base + tb_alloc <= a.out_cap;
-        if (!fits && lane == 0) a.ctl->overflow = 1u;
-        const unsigned long long ob = base + (incl - my);
+        const b9::Reservation r = b9::warp_reserve_bytes(a.out, (tb + 15u) & ~15u, lane);
+        const unsigned long long ob = r.base + (incl - my);
         if (live) {
-            a.out_ids[j] = __ldg(a.ids + slot);
-            a.out_off[j] = fits ? ob : 0; a.out_len[j] = my; a.out_status[j] = rec.status; a.out_has[j] = rec.has;
+            a.out.ids[j] = __ldg(a.ids + slot);
+            b9::store_record(a.out, j, r.fits, ob, my, rec.status, rec.has);
         }
-        if (!fits) continue;
+        if (!r.fits) continue;
         const bool copy = rec.has && rec.mode == b9::EM_COPY;
-        if (rec.has && !copy) b9::endpoint_emit(p, rec, a.out_payload + ob);
+        if (rec.has && !copy) b9::endpoint_emit(p, rec, a.out.payload + ob);
         uint32_t cm = __ballot_sync(0xffffffffu, copy);
         const unsigned long long src = (unsigned long long)(uintptr_t)(p + rec.src_off);
         while (cm) {                                                       // the verbatim records, the whole warp on each
@@ -93,7 +86,7 @@ __global__ void __launch_bounds__(EP_WARPS * 32) endpoint_drain_kernel(b9::Drain
             const uint8_t* s = (const uint8_t*)(uintptr_t)__shfl_sync(0xffffffffu, src, q);
             const unsigned long long d = __shfl_sync(0xffffffffu, ob, q);
             const uint32_t n = __shfl_sync(0xffffffffu, rec.src_len, q);
-            b9::warp_copy(a.out_payload + d, s, n, lane);
+            b9::warp_copy(a.out.payload + d, s, n, lane);
         }
     }
 }

@@ -12,7 +12,7 @@
 // the block's shared memory (28,744 bytes, plus the 1 KiB the SM reserves per block and crc32's 1 KiB table: seven
 // blocks, i.e. seven tasks in flight, per SM). The pass is latency-bound: one thread of each resident warp works, about
 // 900 on a 132-SM H100; scratch in global memory or a warp-cooperative decoder would keep more tasks in flight. Output
-// bytes come from the same control block's cursor.
+// bytes come from the same control block's cursor, one reserve_bytes per task (drain_kernel.cuh).
 #include <stdint.h>
 #include <algorithm>
 #include <cuda_runtime.h>
@@ -44,17 +44,13 @@ __global__ void __launch_bounds__(32) pickle_pass_kernel(b9::DrainArgs a) {
             j = b9::tile_ready_before(a, tile, a.tile_tasks);
             for (uint32_t q = tile * a.tile_tasks; q < i; ++q) j += (b9::hdr_flags(a.hdr[(uint32_t)((a.first_task + q) & a.slot_mask)]) & 1u) ? 0u : 1u;
         }
-        if (a.out_status[j] != b9::ST_UNSUPPORTED) continue;       // drain3_kernel settled it
+        if (a.out.status[j] != b9::ST_UNSUPPORTED) continue;       // drain3_kernel settled it
         const uint8_t* p = a.payload + a.off[(uint32_t)((a.first_task + i) & a.slot_mask)];
         const b9::PkPlan pl = b9::pk_prepare(p, b9::hdr_len(h), H, S, s_crc);
         if (pl.status == b9::ST_UNSUPPORTED) continue;
-        unsigned long long base = 0;
-        const uint32_t alloc = (pl.out_len + 15u) & ~15u;          // the cursor moves in 16-byte units
-        if (alloc) base = atomicAdd(&a.ctl->bytes, (unsigned long long)alloc);
-        const bool fits = base + alloc <= a.out_cap;
-        if (!fits) a.ctl->overflow = 1u;
-        if (fits && pl.out_len) b9::pk_write(p, S, pl, a.out_payload + base);
-        a.out_off[j] = fits ? base : 0; a.out_len[j] = pl.out_len; a.out_status[j] = pl.status; a.out_has[j] = pl.out_len ? 1 : 0;
+        const b9::Reservation r = b9::reserve_bytes(a.out, (pl.out_len + 15u) & ~15u);
+        if (r.fits && pl.out_len) b9::pk_write(p, S, pl, a.out.payload + r.base);
+        b9::store_record(a.out, j, r.fits, r.base, pl.out_len, pl.status, pl.out_len ? 1 : 0);
     }
 }
 

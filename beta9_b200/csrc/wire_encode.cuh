@@ -19,7 +19,7 @@
 //     in Go's map order, duplicates last-wins; HTTP bodies by SerializeHttpPayload's map rules (wire_full_values).
 //     Declines: merged struct kwargs, a literal f64_parse cannot settle, the walk's depth / member limits, TASK_MSG
 //     and PICKLE tasks.
-// One thread per task: a sizing walk, one cursor add per warp, an emitting walk.
+// One thread per task: a sizing walk, one warp_reserve_bytes per warp (drain_kernel.cuh), an emitting walk.
 #pragma once
 #include <stdint.h>
 #ifdef B9_WIRE_ENCODE_HELPERS_ONLY      // tests/host_shim builds the value encoders below for the host
@@ -194,8 +194,7 @@ __device__ __attribute__((noinline)) uint32_t put_dec_ll(uint8_t* o, long long v
 struct WireArgs {
     const uint8_t* payload; const uint64_t* off; const uint64_t* hdr; const uint4* ids; const int64_t* ts; const int64_t* exp;
     uint32_t slot_mask; uint64_t first_task; uint32_t n_tasks;
-    uint8_t* out_payload; uint64_t out_cap; uint64_t* out_off; uint32_t* out_len; uint4* out_ids; uint8_t* out_status; uint8_t* out_has;
-    DrainCtl* ctl;
+    DrainOut out;
 };
 
 // FULL = false: b9_wire_encode; FULL = true: b9_wire_encode_full (the header comment above), instantiated in wire_full.cu
@@ -261,20 +260,14 @@ __global__ void __launch_bounds__(128) wire_encode_kernel(WireArgs a, const Wire
     }
     // one cursor add per warp
     const uint32_t mine = (valid && status == ST_OK) ? total : 0u;
-    uint32_t inc = mine;
-    #pragma unroll
-    for (int d = 1; d < 32; d <<= 1) { uint32_t v = __shfl_up_sync(0xffffffffu, inc, d); if (lane >= d) inc += v; }
-    const uint32_t wtot = __shfl_sync(0xffffffffu, inc, 31);
-    unsigned long long base = 0;
-    if (lane == 0 && wtot) base = atomicAdd(&a.ctl->bytes, (unsigned long long)wtot);
-    base = __shfl_sync(0xffffffffu, base, 0);
-    const bool fits = base + wtot <= a.out_cap;
-    if (!fits && lane == 0) a.ctl->overflow = 1u;
+    const uint32_t inc = warp_incl_scan(mine, lane);
+    const Reservation r = warp_reserve_bytes(a.out, __shfl_sync(0xffffffffu, inc, 31), lane);
     if (!valid) return;
-    const unsigned long long ob = base + (inc - mine);
-    a.out_off[t] = fits ? ob : 0; a.out_len[t] = mine; a.out_ids[t] = a.ids[slot]; a.out_status[t] = (uint8_t)status; a.out_has[t] = mine ? 1 : 0;
-    if (!mine || !fits) return;
-    uint8_t* o = a.out_payload + ob;
+    const unsigned long long ob = r.base + (inc - mine);
+    a.out.ids[t] = a.ids[slot];
+    store_record(a.out, t, r.fits, ob, mine, (uint8_t)status, mine ? 1 : 0);
+    if (!mine || !r.fits) return;
+    uint8_t* o = a.out.payload + ob;
     const char H0[] = "{\"task_id\":\"";
     for (int k = 0; k < 12; ++k) *o++ = (uint8_t)H0[k];
     {

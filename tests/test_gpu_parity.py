@@ -425,6 +425,38 @@ def test_result_capacity_errors_do_not_consume():
         q.close()
 
 
+def test_result_capacity_errors_in_the_identity_tail():
+    """Tasks identity's main loop defers get their bytes in the kernel's tail (both of its branches: JSON payloads, and
+    cloudpickle-framed strings with non-ASCII characters); an overflow there consumes nothing either."""
+    from beta9_b200.device_queue import DeviceQueue
+    from beta9_b200 import _lib as L
+    from oracle.pyoracle import funcloop
+    rng = np.random.default_rng(41)
+    words = ["".join(chr(int(c)) for c in rng.integers(97, 123, int(k))) for k in rng.integers(20, 80, 900)]
+    payloads = [(b'{"args":["%s"]}',                              # compact separators: not the SDK's frame
+                 b'{"args": ["%s\\/x"], "kwargs": {}}',           # an escape json.dumps does not write
+                 b'{"args": [[1, "%s"]], "kwargs": {}}')[i % 3] % w.encode() for i, w in enumerate(words)]
+    b = synth.from_payloads(payloads)
+    o = coracle.run_batch(b.task_ids, b.payload, b.offsets, "identity")
+    assert (o.status == 0).all() and (o.has == 1).all()
+    frames = [funcloop.frame_map_input("café " + w) for w in words]
+    fb = synth.from_payloads(frames)
+    want = [funcloop.run_function_task(f, "identity")[1] for f in frames]
+    cap = 1 << 12
+    for batch, flags, results in ((b, None, [o.result(i) for i in range(b.n)]), (fb, np.full(fb.n, 4, np.uint8), want)):
+        with DeviceQueue(ring_bytes=1 << 22, ring_tasks=1 << 12, max_drain_tasks=1 << 12, max_result_bytes=cap) as q:
+            q.push_batch(batch.task_ids, batch.payload, batch.offsets, flags=flags)
+            with pytest.raises(L.B9Error) as e:
+                q.drain("identity")
+            assert e.value.code == L.B9_ENOSPC and q.depth() == batch.n
+            lens = np.array([len(x) for x in results])
+            k = int(np.searchsorted(np.cumsum((lens + 15) // 16 * 16), cap, side="right"))   # the tail reserves 16-byte units
+            assert 0 < k < batch.n
+            r = q.drain("identity", max_tasks=k)
+            assert r.n == k and q.depth() == batch.n - k and np.array_equal(r.task_ids, batch.task_ids[:k])
+            assert (r.status == 0).all() and [r.result(j) for j in range(k)] == results[:k]
+
+
 # ---- BASELINE.json configs at their stated per-GPU sizes (VERDICT r1: parity was run at reduced sizes for 3 of 4 configs)
 def test_crc32_1m_zipf_full_size():
     """configs[2]: 1M zipf 32..4096-char strings through crc32, every record against the oracle."""

@@ -81,6 +81,23 @@ def test_wire_handcrafted_and_golden(dq):
             assert r.result(i) == want, (name, i)
 
 
+def test_wire_overflow_leaves_the_queue_alone():
+    """Records that exceed max_result_bytes: B9_ENOSPC and nothing consumed; a window that fits is then encoded."""
+    from beta9_b200.device_queue import DeviceQueue
+    from beta9_b200._lib import B9_ENOSPC, B9Error
+    b = synth.strings_batch(2000, 64, adversarial_frac=0.3, seed=13)
+    o = coracle.run_batch(b.task_ids, b.payload, b.offsets, "identity", keep_wire=True, nthreads=8)
+    with DeviceQueue(ring_bytes=1 << 24, ring_tasks=1 << 12, max_drain_tasks=1 << 12, max_result_bytes=1 << 16) as q:
+        push_with_meta(q, b)
+        with pytest.raises(B9Error) as e:
+            q.wire_encode(coracle.DEFAULT_WS, coracle.DEFAULT_STUB, ttl=TTL)
+        assert e.value.code == B9_ENOSPC and q.depth() == b.n
+        r = q.wire_encode(coracle.DEFAULT_WS, coracle.DEFAULT_STUB, ttl=TTL, max_tasks=64)
+        assert r.n == 64 and q.depth() == b.n and np.array_equal(r.task_ids, b.task_ids[:64])
+        assert np.array_equal(r.status, o.status[:64]) and (r.status == 0).sum() > 32
+        assert all(r.result(i) == o.wire_msg(i) for i in range(64) if r.status[i] == 0)
+
+
 def test_wire_sorted_objects_and_kwargs(dq):
     payloads = [loop.sdk_put_payload({"a": 1, "b": [1, 2, {"x": "<", "y": None}], "c": True}, k="v"),
                 loop.sdk_put_payload(a=1, b="é "), loop.sdk_put_payload([{"": 0, "a": -5}]),
