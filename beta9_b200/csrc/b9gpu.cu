@@ -176,6 +176,7 @@ struct b9_ctx {
     // results waiting on the device for b9_drain_fetch
     bool have_results = false, res_peek = false;
     uint32_t res_n = 0, res_popped = 0; uint64_t res_bytes = 0, res_in_bytes = 0; float res_kernel_ms = 0.f;
+    bool res_ids_in_ring = false; uint64_t res_head = 0;   // record j's id is the ring id of task res_head + j (DrainOut::ids_compacted == 0)
     bool expired_since_launch = false, recount_cancelled = false;   // (b9_expire between a launch and its fetch: recount, see b9_drain_fetch)
 
     // ---- multi-GPU (NCCL, loaded with dlopen: the library has no link-time dependency on it)
@@ -230,11 +231,14 @@ bool place_segment(b9_ctx* c, uint64_t bytes, uint64_t* start) {
     return b9_ring_place(c->ring_bytes, !c->segs.empty(), c->segs.empty() ? 0 : c->segs.front().phys_start, c->write_pos, live, bytes, start) != 0;
 }
 
-// the context's result staging, with `ctl` as the control block whose byte cursor places the records' bytes
-DrainOut drain_out(const b9_ctx* c, DrainCtl* ctl) {
+// the context's result staging, with `ctl` as the control block whose byte cursor places the records' bytes. compacted:
+// the launch leaves no record for cancelled slots (count mode), so its records' ids are written to d_out_ids; otherwise
+// they stay in the ring and b9_drain_fetch copies them from there
+DrainOut drain_out(const b9_ctx* c, DrainCtl* ctl, bool compacted) {
     DrainOut o;
     o.payload = c->d_out_payload; o.cap = c->max_result_bytes; o.off = c->d_out_off; o.len = c->d_out_len;
     o.ids = c->d_out_ids; o.status = c->d_out_status; o.has = c->d_out_has; o.ctl = ctl;
+    o.ids_compacted = compacted ? 1u : 0u;
     return o;
 }
 
@@ -999,7 +1003,7 @@ static int64_t drain_launch_common(b9_ctx* c, int handler, uint32_t max_tasks, i
     // the control block: the previous drain kernel zeroed this one (drain_kernel.cuh, D3_CTL_RING), unless something
     // else ran since that the host cannot see through (a failed launch, the wire encoder, the epoch's wrap)
     c->ctl_last = a.epoch % D3_CTL_RING;
-    a.out = drain_out(c, c->d_ctl + c->ctl_last); a.ctl_next = c->d_ctl + (a.epoch + 1u) % D3_CTL_RING;
+    a.out = drain_out(c, c->d_ctl + c->ctl_last, count_mode != 0); a.ctl_next = c->d_ctl + (a.epoch + 1u) % D3_CTL_RING;
     if (c->ctl_dirty) {
         c->last_op_drain = false;
         CU(cudaMemsetAsync(c->d_ctl, 0, D3_CTL_RING * sizeof(DrainCtl), s));
@@ -1053,6 +1057,7 @@ static int64_t drain_launch_common(b9_ctx* c, int handler, uint32_t max_tasks, i
         c->stats.drains++;
     }
     c->res_async = true; c->res_async_n = n; c->res_async_in_bytes = in_bytes;
+    c->res_ids_in_ring = !a.out.ids_compacted; c->res_head = head;        // (a burst of async launches: the last one's records wait)
     if (!c->res_peek) c->running.store(n, std::memory_order_relaxed);
     if (peek & B9_DRAIN_ASYNC) return (int64_t)n;   // records = n minus the cancelled slots: known after b9_sync / b9_drain_fetch
     int rc = finish_launch(c);
@@ -1089,7 +1094,12 @@ int64_t b9_drain_fetch(b9_ctx* c, b9_results* out) {
     if (n) {
         if (!out->task_ids || !out->status || !out->has_result || !out->offsets || !out->lengths) return fail(B9_EINVAL, "b9_drain_fetch: NULL result array");
         CU(cudaMemcpyAsync(out->lengths, c->d_out_len, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
-        CU(cudaMemcpyAsync(out->task_ids, c->d_out_ids, n * 16, cudaMemcpyDeviceToHost, s));
+        if (c->res_ids_in_ring) {                                          // the window's slots: one piece, or two when it wraps the ring
+            const uint32_t slot0 = (uint32_t)(c->res_head & c->slot_mask);
+            const size_t first = std::min<size_t>(n, (size_t)c->slot_mask + 1u - slot0);
+            CU(cudaMemcpyAsync(out->task_ids, c->d_ids + slot0, first * 16, cudaMemcpyDeviceToHost, s));
+            if (first < n) CU(cudaMemcpyAsync(out->task_ids + first * 16, c->d_ids, (n - first) * 16, cudaMemcpyDeviceToHost, s));
+        } else CU(cudaMemcpyAsync(out->task_ids, c->d_out_ids, n * 16, cudaMemcpyDeviceToHost, s));
         CU(cudaMemcpyAsync(out->status, c->d_out_status, n, cudaMemcpyDeviceToHost, s));
         CU(cudaMemcpyAsync(out->has_result, c->d_out_has, n, cudaMemcpyDeviceToHost, s));
         CU(cudaMemcpyAsync(out->offsets, c->d_out_off, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
@@ -1194,7 +1204,8 @@ static int64_t wire_encode(b9_ctx* c, const b9_wire_env* env, uint32_t max_tasks
     WireArgs a{};
     a.payload = c->d_payload; a.off = c->d_off; a.hdr = c->d_hdr; a.ids = c->d_ids; a.ts = c->d_ts; a.exp = c->d_exp;
     a.slot_mask = c->slot_mask; a.first_task = head; a.n_tasks = n;
-    a.out = drain_out(c, c->d_ctl);
+    a.out = drain_out(c, c->d_ctl, false);                                  // (a record for every task of the window)
+    c->res_ids_in_ring = !a.out.ids_compacted; c->res_head = head;
     CU(cudaEventRecord(c->ev_a, s));
     if (full) CU(launch_wire_encode_full(&a, sizeof a, c->d_wire_env, (n + 127) / 128, s));
     else wire_encode_kernel<false><<<(n + 127) / 128, 128, 0, s>>>(a, c->d_wire_env);

@@ -803,17 +803,16 @@ struct D3Warp {
     typename std::conditional<T == 32, D3CopyTab, D3NoTab>::type ct;
 };
 
-struct D3MetaRegs { uint64_t off, hdr; uint4 id; };   // (the id rides along: it is only copied to the record, and loading it a tile ahead takes its latency off the record write)
+struct D3MetaRegs { uint64_t off, hdr; };   // (a record's id is not loaded here: it stays in the ring unless the launch compacts, see DrainOut)
 // tt = tasks per tile of this launch (<= T; the compile-time T for every handler but json_sum)
 template <int T>
 __device__ __forceinline__ void d3_load_meta(const DrainArgs& a, unsigned long long tile, int lane, D3MetaRegs& r, uint32_t tt) {
     const uint32_t t0 = (uint32_t)tile * tt;
-    r.off = 0; r.hdr = 0; r.id = make_uint4(0u, 0u, 0u, 0u);
+    r.off = 0; r.hdr = 0;
     if ((uint32_t)lane < tt && t0 + lane < a.n_tasks) {
         const uint32_t slot = (uint32_t)((a.first_task + t0 + lane) & a.slot_mask);
         r.hdr = __ldg(a.hdr + slot);
         r.off = __ldg(a.off + slot);
-        r.id = __ldg(a.ids + slot);
     }
 }
 
@@ -1309,8 +1308,8 @@ __device__ __noinline__ void slow_task(const DrainArgs& a, uint64_t goff, uint32
     }
     if (!par) {                                                            // the sequential validating parser decides
         if (lane == 0) {
-            // a TaskMessage record: its id is the one the main loop wrote to the record (before it published the item)
-            d2_parse_and_size<0>(p, len, rec, nullptr, http, record ? a.out.ids + j : nullptr);
+            // a TaskMessage record: its id is record j's (in count mode the main loop stored it before it published the item)
+            d2_parse_and_size<0>(p, len, rec, nullptr, http, record ? record_id(a, j) : nullptr);
         }
         rec.src_off = __shfl_sync(0xffffffffu, rec.src_off, 0); rec.src_len = __shfl_sync(0xffffffffu, rec.src_len, 0);
         rec.out_len = __shfl_sync(0xffffffffu, rec.out_len, 0);
@@ -1433,7 +1432,7 @@ __global__ void __launch_bounds__(D3_WARPS * 32, (HANDLER == 1 ? B9_CRC_MINB : H
         return t;
     };
     unsigned long long t_cur = fetch(), t_raw = 0;                         // (q = 0: static on every lane)
-    D3MetaRegs mregs; mregs.off = 0; mregs.hdr = 0; mregs.id = make_uint4(0u, 0u, 0u, 0u);
+    D3MetaRegs mregs; mregs.off = 0; mregs.hdr = 0;
     if (t_cur < a.n_tiles) d3_load_meta<T>(a, t_cur, lane, mregs, TT);
     uint32_t parity = 0;
     bool waited = false;                                                   // grid_dep_wait done (first tile: before its cursor add)
@@ -1450,7 +1449,6 @@ __global__ void __launch_bounds__(D3_WARPS * 32, (HANDLER == 1 ? B9_CRC_MINB : H
         const uint32_t nt = min(TT, a.n_tasks - t0);
         const bool valid = lane < (int)nt;
         const uint64_t m_off = mregs.off;
-        const uint4 m_id = mregs.id;                                       // (lane == task for G == 1)
         const uint32_t m_len = valid ? hdr_len(mregs.hdr) : 0u;
         const bool m_ready = valid && !(hdr_flags(mregs.hdr) & 1u);
         const uint64_t m_end = m_off + m_len;
@@ -1639,7 +1637,7 @@ __global__ void __launch_bounds__(D3_WARPS * 32, (HANDLER == 1 ? B9_CRC_MINB : H
             if (sub == 0) {
                 const uint32_t slot = (uint32_t)((a.first_task + t0 + k) & a.slot_mask);
                 const uint32_t j = base_cnt + ex_cnt;
-                a.out.ids[j] = (G == 1) ? m_id : __ldg(a.ids + slot);
+                store_record_id(a.out, j, a.ids + slot);
                 if (HANDLER == 0 && rec.mode == OM_DEFER) {                // the kernel's tail writes the rest of the record
                     SlowItem* it = a.slow + atomicAdd(&a.out.ctl->n_slow, 1u);
                     it->w1 = (unsigned long long)(my_len | (rec.value == 1 ? 0x80000000u : 0u) | (my_http ? 0x40000000u : 0u)) | ((unsigned long long)j << 32) | (rec.value == 2 ? (1ull << 56) : 0ull)

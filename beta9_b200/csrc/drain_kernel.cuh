@@ -48,17 +48,22 @@ struct SlowItem {
                                     // | bit 57 = a TaskMessage record (B9_TF_TASK_MSG)
 };
 
-// The result records of a drain (or a wire encoding): record j is ids[j], status[j], has[j] and the bytes
+// The result records of a drain (or a wire encoding): record j is its id, status[j], has[j] and the bytes
 // payload[off[j], off[j] + len[j]). Every kernel that writes records places their bytes with reserve_bytes /
-// warp_reserve_bytes and writes the rest with store_record.
+// warp_reserve_bytes and writes the rest with store_record and store_record_id.
+// Where record j's id lives: when the launch compacts its records (a drain in count mode: cancelled slots leave no
+// record), in ids[j]; otherwise record j is the window's task j, and its id stays in that task's ring slot, which nothing
+// writes before the results are fetched (a pop is committed by the fetch): the fetch copies it from there, and no
+// kernel spends 16 bytes of reads and 16 of writes per record on copying it.
 struct DrainOut {
     uint8_t*  payload; uint64_t cap;
     uint64_t* off;                  // [n_tasks + 1]  start of each record's bytes
     uint32_t* len;                  // [n_tasks]      length of each record's bytes
-    uint4*    ids;                  // [n_tasks]
+    uint4*    ids;                  // [n_tasks]      written only when ids_compacted
     uint8_t*  status;               // [n_tasks]
     uint8_t*  has;                  // [n_tasks]
     DrainCtl* ctl;                  // the byte cursor and the overflow flag; for a drain, this launch's entry of the control ring
+    uint32_t  ids_compacted;        // 1: record j's id is ids[j]; 0: it is the ring id of the window's task j
 };
 
 // Result bytes are placed by an atomicAdd on ctl->bytes. A reservation that ends past `cap` sets ctl->overflow (the host
@@ -90,6 +95,11 @@ __device__ __forceinline__ Reservation warp_reserve_bytes(const DrainOut& o, uin
 __device__ __forceinline__ void store_record(const DrainOut& o, uint32_t j, bool fits, unsigned long long off, uint32_t len, uint8_t status, uint8_t has) {
     o.off[j] = fits ? off : 0; o.len[j] = len; o.status[j] = status; o.has[j] = has;
 }
+// record j's id, whose ring slot is `ring_id`: copied to ids[j] only when the launch compacts its records (the id
+// is not even loaded otherwise)
+__device__ __forceinline__ void store_record_id(const DrainOut& o, uint32_t j, const uint4* ring_id) {
+    if (o.ids_compacted) o.ids[j] = __ldg(ring_id);
+}
 
 __device__ __forceinline__ uint32_t warp_incl_scan(uint32_t v, int lane) {
     #pragma unroll
@@ -119,6 +129,11 @@ struct DrainArgs {
     uint32_t static_rounds;         // a worker's first static_rounds tiles are worker + q * workers, the rest come from the ticket counter
     uint32_t tile_tasks;            // json_sum: tasks per warp-tile of THIS launch (4 or 8: small windows balance better on finer tiles); others: fixed
 };
+
+// where record j's id is, once store_record_id has run for it (DrainOut::ids_compacted)
+__device__ __forceinline__ const uint4* record_id(const DrainArgs& a, uint32_t j) {
+    return a.out.ids_compacted ? a.out.ids + j : a.ids + (uint32_t)((a.first_task + j) & a.slot_mask);
+}
 
 constexpr uint32_t TC_SLOTS = 256;             // slots per tile_count_kernel block (8 warps x 32)
 // count_mode: ready tasks before warp-tile `tile` (of T slots) — the record index of its first ready task

@@ -72,7 +72,7 @@ __global__ void __launch_bounds__(EP_WARPS * 32) endpoint_drain_kernel(b9::Drain
         const b9::Reservation r = b9::warp_reserve_bytes(a.out, (tb + 15u) & ~15u, lane);
         const unsigned long long ob = r.base + (incl - my);
         if (live) {
-            a.out.ids[j] = __ldg(a.ids + slot);
+            b9::store_record_id(a.out, j, a.ids + slot);
             b9::store_record(a.out, j, r.fits, ob, my, rec.status, rec.has);
         }
         if (!r.fits) continue;

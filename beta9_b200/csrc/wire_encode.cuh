@@ -264,7 +264,7 @@ __global__ void __launch_bounds__(128) wire_encode_kernel(WireArgs a, const Wire
     const Reservation r = warp_reserve_bytes(a.out, __shfl_sync(0xffffffffu, inc, 31), lane);
     if (!valid) return;
     const unsigned long long ob = r.base + (inc - mine);
-    a.out.ids[t] = a.ids[slot];
+    store_record_id(a.out, t, a.ids + slot);                           // (a no-op: records are 1:1 with the window's tasks)
     store_record(a.out, t, r.fits, ob, mine, (uint8_t)status, mine ? 1 : 0);
     if (!mine || !r.fits) return;
     uint8_t* o = a.out.payload + ob;
