@@ -263,18 +263,17 @@ template <int H> uint32_t drain3_warp_stride(uint32_t in_cap) {
 template <int H> cudaError_t launch_drain3(DrainArgs a, uint64_t avg_task_bytes, uint32_t max_task_len, uint32_t cap_override, int sm_count, bool overlap, cudaStream_t s, int* grid_out,
                                            uint32_t* tt_out) {
     constexpr int T = D3Cfg<H>::T;
-    static const bool tight = !(getenv("B9_STAGE_TIGHT") && atoi(getenv("B9_STAGE_TIGHT")) == 0);      // (=0: the A/B switch)
     uint32_t in_cap = 0, stride = 0; size_t smem = 0; int per_sm = 0;
     // stage buffer per warp sized for the window's average warp-tile: tt tasks x 1.1 + 768 B, within [1 KiB, 48 KiB].
     // Tiles that do not fit are processed straight from global memory (same code, generic loads).
     // (crc32's configuration has long-tailed sizes - zipf strings - and gets a third of a tile of headroom: more would
-    // cost resident warps, and its byte loop lives on those - 16 CTAs per SM fit with this, see B9_CRC_MINB)
+    // cost resident warps, and its byte loop lives on those - 16 CTAs per SM fit with this, see D3Cfg::MIN_BLOCKS)
     auto size_for = [&](uint32_t tt) -> cudaError_t {
         const uint64_t want = (H == B9_H_CRC32) ? avg_task_bytes * tt * 27 / 20 + 768 : avg_task_bytes * tt * 11 / 10 + 768;
         in_cap = (uint32_t)std::min<uint64_t>(48u << 10, std::max<uint64_t>(1u << 10, want));
         // no tile of the window is longer than tt of its longest tasks (+ the alignment of its first byte): with uniform task
         // sizes (configs[3]: every task 372 bytes) the headroom above buys nothing and costs a resident CTA per SM
-        if (tight && H != B9_H_CRC32 && max_task_len) in_cap = (uint32_t)std::min<uint64_t>(in_cap, std::max<uint64_t>(1u << 10, (uint64_t)max_task_len * tt + 32u));
+        if (H != B9_H_CRC32 && max_task_len) in_cap = (uint32_t)std::min<uint64_t>(in_cap, std::max<uint64_t>(1u << 10, (uint64_t)max_task_len * tt + 32u));
         in_cap = (in_cap + 127u) & ~127u;
         if (cap_override) in_cap = cap_override;
         stride = drain3_warp_stride<H>(in_cap);
@@ -292,7 +291,7 @@ template <int H> cudaError_t launch_drain3(DrainArgs a, uint64_t avg_task_bytes,
     // json_sum works on a document with the whole warp: a window of about one 8-document tile per resident warp ends in a
     // ragged last round (configs[4]: 25 k documents per GPU over a few thousand resident warps); tiles of 4 balance it,
     // while larger windows (100 k documents) measured faster with 8
-    if (H == B9_H_JSON_SUM && T >= 8 && (uint64_t)(a.n_tasks + T - 1) / T < 3ull * (uint64_t)per_sm * (uint64_t)sm_count * D3_WARPS) {
+    if (H == B9_H_JSON_SUM && (uint64_t)(a.n_tasks + T - 1) / T < 3ull * (uint64_t)per_sm * (uint64_t)sm_count * D3_WARPS) {
         tt = 4u;
         e = size_for(tt);
         if (e != cudaSuccess) return e;
@@ -306,18 +305,16 @@ template <int H> cudaError_t launch_drain3(DrainArgs a, uint64_t avg_task_bytes,
     // identity with nothing cancelled in the window has a uniform tile cost (its expensive tasks are deferred):
     // all but the last round of a worker's tiles are assigned statically, which measured faster; the same
     // switch made vadd_f32 slower, so it stays on pure work stealing like crc32 / json_sum.
-    // B9_STATIC_ROUNDS=0 turns it off.
-    static const bool allow_static = !(getenv("B9_STATIC_ROUNDS") && atoi(getenv("B9_STATIC_ROUNDS")) == 0);
     if (a.count_mode) {
         e = launch_tile_counts(a, tt, s);
         if (e != cudaSuccess) return e;
     }
-    if (allow_static && H == B9_H_IDENTITY) {
-        // B9_DYNAMIC_ROUNDS: how many of a worker's last rounds come from the ticket counter. One is enough when every
+    if (H == B9_H_IDENTITY) {
+        // dyn: how many of a worker's last rounds come from the ticket counter. One is enough when every
         // tile costs the same; with 1 % of escape-dense strings a tile that holds one takes ~25 % longer (the warp checks its
         // escapes), a worker's static share can hold a dozen of them, and one round of slack does not absorb that: 3 rounds
         // measured faster than 1 on the mix and the same on clean input
-        static const uint64_t dyn = getenv("B9_DYNAMIC_ROUNDS") ? (uint64_t)std::max(1, atoi(getenv("B9_DYNAMIC_ROUNDS"))) : 3u;
+        constexpr uint64_t dyn = 3;
         const uint64_t rounds = a.n_tiles / ((uint64_t)grid * D3_WARPS);
         a.static_rounds = rounds > dyn ? (uint32_t)(rounds - dyn) : 0u;
     }

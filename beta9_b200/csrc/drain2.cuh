@@ -8,7 +8,7 @@
 //   * a warp-tile's payload bytes are ONE contiguous range of the ring in the common case; lane 0
 //     pulls it into the warp's stage buffer with a single bulk async copy (cp.async.bulk / TMA 1-D,
 //     completion on the warp's mbarrier);
-//   * thread per task for identity and vadd_f32 (G = 1): 16-byte shared loads, SWAR classification of
+//   * thread per task for identity and vadd_f32: 16-byte shared loads, SWAR classification of
 //     the string body, 16-byte global stores; the whole warp per task for crc32 and json_sum;
 //   * result RECORDS (id, status, has, offset, length) are FIFO-dense: record j belongs to the j-th
 //     ready task. When no pending task is cancelled (the host knows) j is plain arithmetic on the
@@ -82,26 +82,24 @@ __device__ __forceinline__ uint32_t byte_range_mask(uint32_t word, uint32_t lo, 
     return __vcmpgeu4(idx, lo * 0x01010101u) & __vcmpltu4(idx, hi * 0x01010101u);
 }
 
-// G threads per task (sub = 0..G-1, adjacent lanes): is the payload exactly
+// One thread per task: is the payload exactly
 //   {"args": ["<body>"], "kwargs": {}}
 // with a body of printable ASCII free of '"' and '\\'?  Returns bit0 = frame matches, bit1 = body
-// clean, identical on all G lanes. Must be called by all 32 lanes of the warp (`active` masks the
-// loads of lanes whose task does not exist).
-template <int G>
-__device__ __forceinline__ uint32_t quick_clean_framed(const uint8_t* __restrict__ p, uint32_t len, int sub, bool active) {
+// clean. `active` masks the loads of lanes whose task does not exist.
+__device__ __forceinline__ uint32_t quick_clean_framed(const uint8_t* __restrict__ p, uint32_t len, bool active) {
     uint32_t bad_frame = 0, special = 0;
     if (active && len >= FRAME_PRE_LEN + FRAME_SUF_LEN) {
         // frame: 11 + 17 bytes compared as 32-bit words ("{\"ar" "gs\":" " [\""  /  "\"], " "\"kwa" "rgs\"" ": {}" "}")
         const uint8_t* q = p + len - FRAME_SUF_LEN;
-        if (0 % G == sub) bad_frame |= ld_u32_unaligned(p) != 0x7261227Bu;
-        if (1 % G == sub) bad_frame |= ld_u32_unaligned(p + 4) != 0x3A227367u;
-        if (2 % G == sub) bad_frame |= (ld_u32_unaligned(p + 8) & 0x00FFFFFFu) != 0x00225B20u;
-        if (3 % G == sub) bad_frame |= ld_u32_unaligned(q) != 0x202C5D22u;
-        if (4 % G == sub) bad_frame |= ld_u32_unaligned(q + 4) != 0x61776B22u;
-        if (5 % G == sub) bad_frame |= ld_u32_unaligned(q + 8) != 0x22736772u;
-        if (6 % G == sub) bad_frame |= ld_u32_unaligned(q + 12) != 0x7D7B203Au;
-        if (7 % G == sub) bad_frame |= q[16] != '}';
-        // body = [b0, b1): aligned 16-byte groups, group i handled by lane i % G; bytes of the first /
+        bad_frame |= ld_u32_unaligned(p) != 0x7261227Bu;
+        bad_frame |= ld_u32_unaligned(p + 4) != 0x3A227367u;
+        bad_frame |= (ld_u32_unaligned(p + 8) & 0x00FFFFFFu) != 0x00225B20u;
+        bad_frame |= ld_u32_unaligned(q) != 0x202C5D22u;
+        bad_frame |= ld_u32_unaligned(q + 4) != 0x61776B22u;
+        bad_frame |= ld_u32_unaligned(q + 8) != 0x22736772u;
+        bad_frame |= ld_u32_unaligned(q + 12) != 0x7D7B203Au;
+        bad_frame |= q[16] != '}';
+        // body = [b0, b1): aligned 16-byte groups; bytes of the first /
         // last group outside the body are replaced by 'a' before the SWAR test. (A garbage frame makes
         // the answer irrelevant, but the loads stay inside the payload: len >= 28.)
         const uint8_t* b0 = p + FRAME_PRE_LEN;
@@ -112,7 +110,7 @@ __device__ __forceinline__ uint32_t quick_clean_framed(const uint8_t* __restrict
         const uint32_t lead = (uint32_t)(b0 - g0);                  // bytes to ignore at the front of the first group
         const uint32_t tail_keep = 16u - (uint32_t)(g1 - b1);       // bytes to keep in the last group
         const uint32_t A = 0x61616161u;
-        for (const uint8_t* g = g0 + 16 * sub; g < g1; g += 16 * G) {
+        for (const uint8_t* g = g0; g < g1; g += 16) {
             uint4 v = *(const uint4*)g;
             const bool first = g == g0, last = g + 16 == g1;
             if (first | last) {
@@ -126,9 +124,7 @@ __device__ __forceinline__ uint32_t quick_clean_framed(const uint8_t* __restrict
             special |= swar_special16(v.x, v.y, v.z, v.w) ? 1u : 0u;
         }
     } else bad_frame = 1;
-    uint32_t bits = bad_frame | (special << 1);
-    #pragma unroll
-    for (int d = 1; d < G; d <<= 1) bits |= __shfl_xor_sync(0xffffffffu, bits, d);
+    const uint32_t bits = bad_frame | (special << 1);
     return (bits & 1u ? 0u : 1u) | (bits & 2u ? 0u : 2u);
 }
 
@@ -150,22 +146,21 @@ __device__ __forceinline__ void copy_small_down(uint8_t* __restrict__ dst, const
     if (n & 1u) dst[i] = src[i];
 }
 
-// Copy of n bytes to global memory by the G threads of a task: 16-byte stores on the destination
-// (vector v by lane v % G), 4-byte loads + funnel shift on the (arbitrarily aligned) source.
-template <int G>
-__device__ __forceinline__ void group_copy(uint8_t* __restrict__ dst, const uint8_t* __restrict__ src, uint32_t n, int sub) {
+// Copy of n bytes to global memory by the task's thread: 16-byte stores on the destination,
+// 4-byte loads + funnel shift on the (arbitrarily aligned) source.
+__device__ __forceinline__ void group_copy(uint8_t* __restrict__ dst, const uint8_t* __restrict__ src, uint32_t n) {
     uint32_t head = (uint32_t)((16u - ((uintptr_t)dst & 15u)) & 15u);
     if (head > n) {                                              // tiny copy that never reaches an aligned vector
-        if (sub == 0) for (uint32_t i = 0; i < n; ++i) dst[i] = src[i];
+        for (uint32_t i = 0; i < n; ++i) dst[i] = src[i];
         return;
     }
-    if (sub == 0) copy_small_up(dst, src, head);
+    copy_small_up(dst, src, head);
     dst += head; src += head; n -= head;
     const uint32_t nvec = n >> 4;
     const uint32_t sh = (uint32_t)((uintptr_t)src & 3u), bits = sh * 8;
     const uint32_t* sw = (const uint32_t*)(src - sh);
     uint4* dv = (uint4*)dst;
-    for (uint32_t v = sub; v < nvec; v += G) {
+    for (uint32_t v = 0; v < nvec; ++v) {
         const uint32_t* s4 = sw + 4 * v;
         const uint32_t w0 = s4[0], w1 = s4[1], w2 = s4[2], w3 = s4[3], w4 = s4[4];   // w4: <= 3 bytes of over-read, inside the buffers' slack
         uint4 o;
@@ -173,7 +168,8 @@ __device__ __forceinline__ void group_copy(uint8_t* __restrict__ dst, const uint
         o.z = __funnelshift_r(w2, w3, bits); o.w = __funnelshift_r(w3, w4, bits);
         dv[v] = o;
     }
-    if (sub == G - 1) { const uint32_t done = nvec << 4; copy_small_down(dst + done, src + done, n - done); }
+    const uint32_t done = nvec << 4;
+    copy_small_down(dst + done, src + done, n - done);
 }
 
 // ------------------------------------------------------------------ chunk-parallel string transcoding
@@ -771,18 +767,15 @@ __device__ __forceinline__ int json_sum_coop(const uint8_t* __restrict__ p, uint
 // time at __syncthreads behind warp 0's staging, the cursor atomic and the escaped-string pass.)
 constexpr int D3_WARPS = 2;                  // warps per CTA (a container only)
 template <int HANDLER> struct D3Cfg {
-    // threads per task. G = 2 doubles the warps per staged byte but also doubles the per-task setup
-    // instructions (both lanes execute them); with no barriers to hide, G = 1 wins.
-#ifndef B9_IDENTITY_G
-#define B9_IDENTITY_G 1
-#endif
-    static constexpr int G = (HANDLER == 0) ? B9_IDENTITY_G : 1;
-    // tasks per warp-tile. crc32 (configs[2]: zipf 32..4096-byte strings, ~1 KB on average) works on a task
-    // with the whole warp, so its tiles are small: 4 tasks keep the stage buffer at ~5 KB, which leaves L1 room for the shift tables.
-#ifndef B9_JSON_T
-#define B9_JSON_T 8
-#endif
-    static constexpr int T = (HANDLER == 1) ? 4 : (HANDLER == 3) ? B9_JSON_T : 32 / G;
+    // tasks per warp-tile. Identity and vadd_f32 run one thread per task (two lanes per task doubled the per-task setup,
+    // which both lanes execute, and measured slower). crc32 (configs[2]: zipf 32..4096-byte strings, ~1 KB on average)
+    // works on a task with the whole warp, so its tiles are small: 4 tasks keep the stage buffer at ~5 KB, which leaves
+    // L1 room for the shift tables. json_sum also works on a task with the whole warp (8, or 4 for small windows: launch_drain3).
+    static constexpr int T = (HANDLER == 1) ? 4 : (HANDLER == 3) ? 8 : 32;
+    // resident CTAs per SM the register allocation aims for. crc32's byte loop waits on its table loads and more warps hide
+    // them: it ran fastest with 64 registers / 16 CTAs and a stage buffer that lets 16 fit (fewer CTAs with more registers
+    // were slower at every step from 10 to 16). identity is limited to 9 CTAs by its stage buffers, not by registers.
+    static constexpr int MIN_BLOCKS = (HANDLER == 1) ? 16 : 9;
 };
 constexpr int D2_THREADS = 4;                // host: the smallest warp-tile (sizes the per-tile count arrays)
 
@@ -878,17 +871,9 @@ __device__ __noinline__ uint32_t d3_stage_scattered(const uint8_t* __restrict__ 
 }
 
 // out-of-line generic-pointer versions for tiles that could not be staged (and other cold paths)
-template <int G>
-__device__ __noinline__ uint32_t quick_clean_framed_generic(const uint8_t* p, uint32_t len, int sub, bool active) { return quick_clean_framed<G>(p, len, sub, active); }
-template <int G>
-__device__ __noinline__ void group_copy_staged(uint8_t* dst, const uint8_t* src, uint32_t n, int sub) { group_copy<G>(dst, src, n, sub); }   // (tiles the coalesced copy does not take)
-template <int G>
-__device__ __noinline__ void group_copy_generic(uint8_t* dst, const uint8_t* src, uint32_t n, int sub) { group_copy<G>(dst, src, n, sub); }
-
-// (identity's main loop never holds a float64 / container record: those tasks are deferred to slow_task, which calls
-// seq_emit<true> itself; leaving the call out of the loop keeps configs[1]'s kernel as it was)
-template <int HANDLER>
-__device__ __forceinline__ void d2_phase_b_task(const uint8_t* __restrict__ p, const TaskRec& rec, uint8_t* __restrict__ o) { seq_emit<HANDLER == 3>(p, rec, o); }
+__device__ __noinline__ uint32_t quick_clean_framed_generic(const uint8_t* p, uint32_t len, bool active) { return quick_clean_framed(p, len, active); }
+__device__ __noinline__ void group_copy_staged(uint8_t* dst, const uint8_t* src, uint32_t n) { group_copy(dst, src, n); }   // (tiles the coalesced copy does not take)
+__device__ __noinline__ void group_copy_generic(uint8_t* dst, const uint8_t* src, uint32_t n) { group_copy(dst, src, n); }
 
 // the sequential validating parser + handler sizing, out of line: rare for identity, and it keeps the
 // hot loops' registers and instruction-cache footprint small. record: the bytes are a TaskMessage record
@@ -1370,20 +1355,8 @@ __device__ __noinline__ void d3_identity_tail(const DrainArgs& a, uint8_t* __res
 }
 
 template <int HANDLER>
-// resident CTAs per SM the register allocation aims for. crc32's byte loop waits on its table loads and more warps hide
-// them: it ran fastest with 64 registers / 16 CTAs and a stage buffer that lets 16 fit (fewer CTAs with more registers
-// were slower at every step from 10 to 16). identity is limited to 9 CTAs by its stage buffers, not by registers.
-#ifndef B9_CRC_MINB
-#define B9_CRC_MINB 16
-#endif
-#ifndef B9_VADD_MINB
-#define B9_VADD_MINB 9
-#endif
-#ifndef B9_JSON_MINB
-#define B9_JSON_MINB 9
-#endif
-__global__ void __launch_bounds__(D3_WARPS * 32, (HANDLER == 1 ? B9_CRC_MINB : HANDLER == 2 ? B9_VADD_MINB : HANDLER == 3 ? B9_JSON_MINB : 9)) drain3_kernel(DrainArgs a, uint32_t in_cap, uint32_t warp_stride) {
-    constexpr int G = D3Cfg<HANDLER>::G, T = D3Cfg<HANDLER>::T;
+__global__ void __launch_bounds__(D3_WARPS * 32, D3Cfg<HANDLER>::MIN_BLOCKS) drain3_kernel(DrainArgs a, uint32_t in_cap, uint32_t warp_stride) {
+    constexpr int T = D3Cfg<HANDLER>::T;
     const uint32_t TT = (HANDLER == 3) ? a.tile_tasks : (uint32_t)T;      // tasks per tile: json_sum's is chosen per launch (<= T)
     extern __shared__ __align__(128) uint8_t d3_smem[];
     __shared__ uint32_t s_crc_table[HANDLER == 1 ? 256 : 1];
@@ -1393,7 +1366,6 @@ __global__ void __launch_bounds__(D3_WARPS * 32, (HANDLER == 1 ? B9_CRC_MINB : H
     uint8_t* const wbase = d3_smem + (size_t)warp * warp_stride;
     D3Warp<T>& W = *reinterpret_cast<D3Warp<T>*>(wbase);
     uint8_t* const sbuf = wbase + ((sizeof(D3Warp<T>) + 127u) & ~127u);   // stage buffer (+64 bytes of readable slack)
-    const int k = lane / G, sub = lane % G;                                // my task inside the warp-tile, my share of it
 
     // Back-to-back drains overlap (programmatic dependent launch, see the host's launch_drain3): the next drain's CTAs may
     // become resident as soon as this grid's leave. Until its grid_dep_wait a warp touches only what no drain writes — slot
@@ -1477,13 +1449,13 @@ __global__ void __launch_bounds__(D3_WARPS * 32, (HANDLER == 1 ? B9_CRC_MINB : H
         __syncwarp();                                                     // W.* visible to all lanes
         if (staged) { mbar_wait(&W.mbar, parity); parity ^= 1u; }
 
-        // ---------------- phase A: G lanes per task ----------------------------------------------------
-        const bool mine = k < (int)nt && ((ready_mask_t >> k) & 1u);
-        const uint32_t my_len = mine ? W.len[k] : 0u;
-        const uint32_t my_soff = (mine && staged) ? W.soff[k] : 0u;
-        const uint64_t my_goff = mine ? W.goff[k] : 0ull;
-        const bool my_http = mine && (W.flg[k] & B9_TF_HTTP_BODY_BIT) != 0;
-        const bool my_pickle = mine && (W.flg[k] & B9_TF_PICKLE_BIT) != 0;
+        // ---------------- phase A: one lane per task (identity, vadd_f32) or the whole warp per task -----
+        const bool mine = lane < (int)nt && ((ready_mask_t >> lane) & 1u);
+        const uint32_t my_len = mine ? W.len[lane] : 0u;
+        const uint32_t my_soff = (mine && staged) ? W.soff[lane] : 0u;
+        const uint64_t my_goff = mine ? W.goff[lane] : 0ull;
+        const bool my_http = mine && (W.flg[lane] & B9_TF_HTTP_BODY_BIT) != 0;
+        const bool my_pickle = mine && (W.flg[lane] & B9_TF_PICKLE_BIT) != 0;
         TaskRec rec; rec.ready = mine; rec.status = 0; rec.has = 0; rec.mode = OM_NONE; rec.out_len = 0; rec.src_off = 0; rec.src_len = 0; rec.value = 0;
         bool clobbered = false;
         if (HANDLER == 0) {
@@ -1491,8 +1463,8 @@ __global__ void __launch_bounds__(D3_WARPS * 32, (HANDLER == 1 ? B9_CRC_MINB : H
             // json.dumps); everything else is put on the work list of the kernel's tail (d3_identity_tail), so that
             // this loop stays small enough for the instruction cache and no worker stalls on a 1 % case
             uint32_t q;
-            if (staged) q = quick_clean_framed<G>(sbuf + my_soff, my_len, sub, mine);
-            else        q = quick_clean_framed_generic<G>(a.payload + my_goff, my_len, sub, mine);
+            if (staged) q = quick_clean_framed(sbuf + my_soff, my_len, mine);
+            else        q = quick_clean_framed_generic(a.payload + my_goff, my_len, mine);
             if (mine) {
                 if (q == 3u) {
                     const uint32_t tok = my_len - FRAME_PRE_LEN - FRAME_SUF_LEN + 2;
@@ -1514,12 +1486,12 @@ __global__ void __launch_bounds__(D3_WARPS * 32, (HANDLER == 1 ? B9_CRC_MINB : H
                         }
                     }
                 }
-                if (W.flg[k] & B9_TF_TASK_MSG_BIT) {                       // a TaskMessage record: the kernel's tail, unless the check below settles it
+                if (W.flg[lane] & B9_TF_TASK_MSG_BIT) {                    // a TaskMessage record: the kernel's tail, unless the check below settles it
                     rec.has = 0; rec.out_len = 0; rec.mode = OM_DEFER; rec.value = 3;
                     if (my_http || my_pickle) { rec.mode = OM_NONE; rec.value = 0; rec.status = ST_UNSUPPORTED; }   // no record is either
                 }
             }
-            if constexpr (HANDLER == 0 && T == 32) {
+            if constexpr (HANDLER == 0) {
                 // framed, but the body holds escapes: the warp checks that they are json.dumps's own (then the task is a copy after all)
                 uint32_t dirty = staged ? __ballot_sync(0xffffffffu, mine && rec.mode == OM_DEFER && rec.value == 1) : 0u;
                 while (dirty) {
@@ -1537,7 +1509,7 @@ __global__ void __launch_bounds__(D3_WARPS * 32, (HANDLER == 1 ? B9_CRC_MINB : H
                 const bool my_rec = mine && rec.mode == OM_DEFER && rec.value == 3;
                 if (__any_sync(0xffffffffu, my_rec)) {
                     unsigned long long qm = 0;
-                    if (my_rec && staged) qm = task_msg_quick(sbuf + my_soff, my_len, a.ids + ((a.first_task + t0 + k) & a.slot_mask));
+                    if (my_rec && staged) qm = task_msg_quick(sbuf + my_soff, my_len, a.ids + ((a.first_task + t0 + lane) & a.slot_mask));
                     const uint32_t ts = (uint32_t)qm, tl = (uint32_t)(qm >> 32) & 0x7FFFFFFFu;
                     if (qm && !(qm >> 63)) {
                         rec.mode = OM_NONE; rec.value = 0;                       // "" is falsy
@@ -1589,12 +1561,12 @@ __global__ void __launch_bounds__(D3_WARPS * 32, (HANDLER == 1 ? B9_CRC_MINB : H
             rec.status = ST_UNSUPPORTED;                                   // function path: identity only
         } else if (mine) {
             int fr = 0;
-            const bool my_rec = (W.flg[k] & B9_TF_TASK_MSG_BIT) != 0;
+            const bool my_rec = (W.flg[lane] & B9_TF_TASK_MSG_BIT) != 0;
             if (HANDLER == 2 && staged && !my_http && !my_rec) fr = vadd_fast(sbuf + my_soff, my_len, s_b64, rec);
             if (fr != 1) {
                 clobbered = fr == 2;                                       // stage bytes overwritten: read the ring instead
                 const uint8_t* p = (staged && !clobbered) ? (const uint8_t*)(sbuf + my_soff) : a.payload + my_goff;
-                if (my_rec) d2_parse_and_size<HANDLER>(p, my_len, rec, s_crc_table, my_http, a.ids + ((a.first_task + t0 + k) & a.slot_mask));
+                if (my_rec) d2_parse_and_size<HANDLER>(p, my_len, rec, s_crc_table, my_http, a.ids + ((a.first_task + t0 + lane) & a.slot_mask));
                 else        d2_parse_and_size<HANDLER>(p, my_len, rec, s_crc_table, my_http);
             }
         }
@@ -1610,16 +1582,14 @@ __global__ void __launch_bounds__(D3_WARPS * 32, (HANDLER == 1 ? B9_CRC_MINB : H
         if (lane == 0 && tile == a.n_tiles - 1) a.out.ctl->total_cnt = base_cnt + rc;
 
         // ---------------- compaction (ballot) + sizes (scan) + ONE cursor add per warp-tile -------------
-        const uint32_t my_bytes = (sub == 0) ? rec.out_len : 0u;
-        const uint32_t ex_bytes0 = warp_excl_scan(my_bytes, lane);
-        const uint32_t tb = __shfl_sync(0xffffffffu, ex_bytes0 + my_bytes, 31);
-        const uint32_t ex_bytes = __shfl_sync(0xffffffffu, ex_bytes0, k * G);      // every lane of a task sees the task's offset
-        const uint32_t ex_cnt = __popc(ready_mask_t & ((1u << k) - 1u));
+        const uint32_t ex_bytes = warp_excl_scan(rec.out_len, lane);
+        const uint32_t tb = __shfl_sync(0xffffffffu, ex_bytes + rec.out_len, 31);
+        const uint32_t ex_cnt = __popc(ready_mask_t & ((1u << lane) - 1u));
         // thread-per-task handlers reserve whole 16-byte units, so that every tile's range starts on a vector
         // boundary (the coalesced copy below); the <= 15 bytes of padding per tile are never referenced by a record
         // (identity only: for vadd_f32, whose kernel is bound by the base64 arithmetic, the warp-wide copy's extra
         // instructions cost more than its coalescing saves: it measured slower)
-        constexpr bool COAL = (T == 32 && G == 1 && HANDLER == 0);
+        constexpr bool COAL = HANDLER == 0;
         const Reservation res = warp_reserve_bytes(a.out, COAL ? ((tb + 15u) & ~15u) : tb, lane);
         const unsigned long long base = res.base;
         const bool fits = res.fits;
@@ -1628,32 +1598,32 @@ __global__ void __launch_bounds__(D3_WARPS * 32, (HANDLER == 1 ? B9_CRC_MINB : H
             const uint32_t c_len = (mine && rec.has && rec.mode == OM_COPY) ? rec.src_len : 0u;
             const bool ok_me = rec.out_len == c_len && (c_len == 0u || c_len >= 16u);
             coal = staged && fits && tb != 0u && tb <= D3_COPY_MAX_BYTES && __all_sync(0xffffffffu, ok_me);
-            if (coal) d3_copy_tile(W.ct, sbuf, a.out.payload + base, c_len, ex_bytes0, my_soff + rec.src_off, tb, lane);
+            if (coal) d3_copy_tile(W.ct, sbuf, a.out.payload + base, c_len, ex_bytes, my_soff + rec.src_off, tb, lane);
         }
 
-        // ---------------- phase B: G lanes per task ----------------------------------------------------
+        // ---------------- phase B: the task's lane writes its record and bytes --------------------------
         if (mine) {
             const uint64_t ob = base + ex_bytes;
-            if (sub == 0) {
-                const uint32_t slot = (uint32_t)((a.first_task + t0 + k) & a.slot_mask);
-                const uint32_t j = base_cnt + ex_cnt;
-                store_record_id(a.out, j, a.ids + slot);
-                if (HANDLER == 0 && rec.mode == OM_DEFER) {                // the kernel's tail writes the rest of the record
-                    SlowItem* it = a.slow + atomicAdd(&a.out.ctl->n_slow, 1u);
-                    it->w1 = (unsigned long long)(my_len | (rec.value == 1 ? 0x80000000u : 0u) | (my_http ? 0x40000000u : 0u)) | ((unsigned long long)j << 32) | (rec.value == 2 ? (1ull << 56) : 0ull)
-                           | (rec.value == 3 ? (1ull << 57) : 0ull);
-                    __threadfence();
-                    *(volatile unsigned long long*)&it->w0 = my_goff | ((unsigned long long)a.epoch << 40);
-                } else store_record(a.out, j, fits, ob, rec.out_len, rec.status, rec.has);
-            }
+            const uint32_t slot = (uint32_t)((a.first_task + t0 + lane) & a.slot_mask);
+            const uint32_t j = base_cnt + ex_cnt;
+            store_record_id(a.out, j, a.ids + slot);
+            if (HANDLER == 0 && rec.mode == OM_DEFER) {                    // the kernel's tail writes the rest of the record
+                SlowItem* it = a.slow + atomicAdd(&a.out.ctl->n_slow, 1u);
+                it->w1 = (unsigned long long)(my_len | (rec.value == 1 ? 0x80000000u : 0u) | (my_http ? 0x40000000u : 0u)) | ((unsigned long long)j << 32) | (rec.value == 2 ? (1ull << 56) : 0ull)
+                       | (rec.value == 3 ? (1ull << 57) : 0ull);
+                __threadfence();
+                *(volatile unsigned long long*)&it->w0 = my_goff | ((unsigned long long)a.epoch << 40);
+            } else store_record(a.out, j, fits, ob, rec.out_len, rec.status, rec.has);
             if (rec.has && fits) {
                 if (rec.mode == OM_COPY) {
                     if (coal) {}                                            // written by d3_copy_tile
-                    else if (staged) group_copy_staged<G>(a.out.payload + ob, sbuf + my_soff + rec.src_off, rec.src_len, sub);
-                    else             group_copy_generic<G>(a.out.payload + ob, a.payload + my_goff + rec.src_off, rec.src_len, sub);
-                } else if (sub == 0 && rec.mode != OM_STR_PAR) {
+                    else if (staged) group_copy_staged(a.out.payload + ob, sbuf + my_soff + rec.src_off, rec.src_len);
+                    else             group_copy_generic(a.out.payload + ob, a.payload + my_goff + rec.src_off, rec.src_len);
+                } else if (rec.mode != OM_STR_PAR) {
+                    // (identity's main loop never holds a float64 / container record: those tasks are deferred to slow_task, which
+                    // calls seq_emit<true> itself; leaving the call out of the loop keeps configs[1]'s kernel as it was)
                     const uint8_t* p = (staged && !clobbered) ? (const uint8_t*)(sbuf + my_soff) : a.payload + my_goff;
-                    d2_phase_b_task<HANDLER>(p, rec, a.out.payload + ob);
+                    seq_emit<HANDLER == 3>(p, rec, a.out.payload + ob);
                 }
             }
         }
