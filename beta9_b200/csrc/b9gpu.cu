@@ -6,6 +6,7 @@
 // the reference's FIFO Redis list (pkg/abstractions/taskqueue/client.go:29-96: RPUSH at the tail,
 // LPOP at the head) with `RingBuffer`-style fixed capacity (pkg/abstractions/common/ring_buffer.go).
 #include <cuda_runtime.h>
+#include <cub/device/device_scan.cuh>
 
 #include <algorithm>
 #include <cmath>
@@ -143,6 +144,13 @@ struct b9_ctx {
     // push staging (device): raw offsets + optional metadata of the batch being ingested
     uint64_t* d_in_off = nullptr; int64_t* d_in_ts = nullptr; int64_t* d_in_exp = nullptr;
     uint8_t*  d_in_retries = nullptr; uint8_t* d_in_flags = nullptr;
+    // the retry policy (b9_set_retry_policy; set under out_mu) and the re-push's device buffers (allocated with the first policy)
+    uint32_t retry_mask = 0, max_retries = 0;
+    uint32_t* d_task_of = nullptr;             // [max_drain_tasks] DrainArgs::task_of
+    uint32_t* d_retry_rec = nullptr;           // [max_drain_tasks] the RETRY records of a fetch, in record order
+    uint4* d_retry_ids = nullptr;              // [max_drain_tasks] their ids
+    uint8_t* d_retry_bytes = nullptr; uint64_t retry_bytes_cap = 0;   // their payload bytes (grow-only)
+    void* d_retry_scan = nullptr; size_t retry_scan_cap = 0;          // cub scan scratch (grow-only)
     // ring bookkeeping (host)
     uint64_t head_task = 0, tail_task = 0;     // logical, monotonically increasing
     uint64_t write_pos = 0;                    // physical byte position of the next segment
@@ -175,6 +183,8 @@ struct b9_ctx {
     unsigned long long* d_count = nullptr; unsigned long long* h_count = nullptr;
     // results waiting on the device for b9_drain_fetch
     bool have_results = false, res_peek = false;
+    bool res_retry = false;                    // the waiting results come from a drain launched under a retry policy
+    uint64_t res_gen = 0;                      // bumped whenever the waiting results change (launch, fetch commit)
     uint32_t res_n = 0, res_popped = 0; uint64_t res_bytes = 0, res_in_bytes = 0; float res_kernel_ms = 0.f;
     bool res_ids_in_ring = false; uint64_t res_head = 0;   // record j's id is the ring id of task res_head + j (DrainOut::ids_compacted == 0)
     bool expired_since_launch = false, recount_cancelled = false;   // (b9_expire between a launch and its fetch: recount, see b9_drain_fetch)
@@ -264,6 +274,7 @@ template <int H> cudaError_t launch_drain3(DrainArgs a, uint64_t avg_task_bytes,
                                            uint32_t* tt_out) {
     constexpr int T = D3Cfg<H>::T;
     uint32_t in_cap = 0, stride = 0; size_t smem = 0; int per_sm = 0;
+    void (*const kernel)(DrainArgs, uint32_t, uint32_t) = a.retry_mask ? drain3_kernel<H, true> : drain3_kernel<H, false>;
     // stage buffer per warp sized for the window's average warp-tile: tt tasks x 1.1 + 768 B, within [1 KiB, 48 KiB].
     // Tiles that do not fit are processed straight from global memory (same code, generic loads).
     // (crc32's configuration has long-tailed sizes - zipf strings - and gets a third of a tile of headroom: more would
@@ -278,9 +289,9 @@ template <int H> cudaError_t launch_drain3(DrainArgs a, uint64_t avg_task_bytes,
         if (cap_override) in_cap = cap_override;
         stride = drain3_warp_stride<H>(in_cap);
         smem = (size_t)stride * D3_WARPS;
-        cudaError_t e = cudaFuncSetAttribute(drain3_kernel<H>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
-        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, drain3_kernel<H>, D3_WARPS * 32, smem);
+        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, D3_WARPS * 32, smem);
         if (e != cudaSuccess) return e;
         if (per_sm < 1) per_sm = 1;
         return cudaSuccess;
@@ -325,7 +336,7 @@ template <int H> cudaError_t launch_drain3(DrainArgs a, uint64_t avg_task_bytes,
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr; cfg.numAttrs = (overlap && !a.count_mode) ? 1 : 0;
-    e = cudaLaunchKernelEx(&cfg, drain3_kernel<H>, a, in_cap, stride);
+    e = cudaLaunchKernelEx(&cfg, kernel, a, in_cap, stride);
     if (e != cudaSuccess) return e;
     return cudaGetLastError();
 }
@@ -389,11 +400,193 @@ int recount_cancelled_locked_out(b9_ctx* c) {
     return B9_OK;
 }
 
+// Commits the pop of the fetched window (the head moves past it, its fully consumed segments are freed). Caller holds c->mu.
+void commit_pop(b9_ctx* c) {
+    c->head_task += c->res_popped; c->pending_bytes -= c->res_in_bytes; c->stats.tasks_drained += c->res_popped;
+    c->cancelled_pending -= std::min<uint64_t>(c->cancelled_pending, (uint64_t)(c->res_popped - c->res_n));
+    c->recount_cancelled = c->expired_since_launch;              // an expire ran between this drain's launch and its commit: its
+                                                                  // count included tasks of the window that are gone now
+    free_segments(c);
+}
+
+// The re-push's device half, for retried task k = the window task (task_of) of record rec[k]. retry_len_kernel, one thread
+// per task: rel[k + 1] = its length (a scan then makes rel the exclusive byte prefix). retry_gather_kernel, one warp per
+// task: its bytes are copied out of the claimed window into the scratch `bytes` at rel[k], with the slot words
+// ingest_kernel writes for a push: retries + 1, the commit's timestamp, the same expiry, flags and id.
+__global__ void retry_len_kernel(const uint32_t* __restrict__ rec, uint32_t n, const uint32_t* __restrict__ task_of, const uint64_t* __restrict__ hdr,
+                                 uint64_t head, uint32_t slot_mask, uint64_t* __restrict__ rel) {
+    const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k == 0) rel[0] = 0;
+    if (k < n) rel[k + 1] = hdr_len(hdr[(uint32_t)((head + task_of[rec[k]]) & slot_mask)]);
+}
+__global__ void retry_gather_kernel(const uint32_t* __restrict__ rec, uint32_t n, const uint32_t* __restrict__ task_of, uint64_t head, uint32_t slot_mask,
+                                    const uint8_t* __restrict__ payload, const uint64_t* __restrict__ off, const uint64_t* __restrict__ hdr,
+                                    const uint4* __restrict__ ids, const int64_t* __restrict__ exp, const uint64_t* __restrict__ rel, int64_t now_unix,
+                                    uint8_t* __restrict__ bytes, int64_t* __restrict__ o_ts, int64_t* __restrict__ o_exp, uint8_t* __restrict__ o_retries,
+                                    uint8_t* __restrict__ o_flags, uint4* __restrict__ o_ids) {
+    const uint32_t k = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31u;
+    if (k >= n) return;
+    const uint32_t slot = (uint32_t)((head + task_of[rec[k]]) & slot_mask);
+    const uint64_t h = hdr[slot];
+    warp_copy(bytes + rel[k], payload + off[slot], hdr_len(h), (int)lane);
+    if (lane == 0) {
+        o_ts[k] = now_unix; o_exp[k] = exp[slot]; o_retries[k] = (uint8_t)(hdr_retries(h) + 1u); o_flags[k] = (uint8_t)hdr_flags(h); o_ids[k] = ids[slot];
+    }
+}
+
+// b9_drain_fetch's commit when records are RETRY: the pop and the re-push of those tasks at the tail (Dispatcher.RetryTask's
+// RPUSH, pkg/task/dispatch.go:232-285). Caller holds c->in_mu (the re-push is a push) and c->out_mu, and the records are
+// fetched. Everything runs on the ingest stream, behind earlier pushes and ahead of later ones: the tasks are gathered out
+// of the claimed window into scratch, then the space is placed in the same critical section that commits the pop (a
+// producer cannot take the released space in between), then the bytes and slot words go to the new segment. When the
+// ring has no room for it, nothing is committed: B9_ENOSPC.
+int commit_with_repush(b9_ctx* c, const std::vector<uint32_t>& retry_rec, float d2h_ms) {
+    const uint32_t k = (uint32_t)retry_rec.size();
+    cudaStream_t s = c->stream_in;
+    const uint64_t head = c->res_head;
+    if (c->retry_bytes_cap < c->res_in_bytes) {                            // (the retried bytes are at most the window's)
+        cudaFree(c->d_retry_bytes); c->d_retry_bytes = nullptr; c->retry_bytes_cap = 0;
+        const cudaError_t e = cudaMalloc(&c->d_retry_bytes, c->res_in_bytes + RING_SLACK);
+        if (e != cudaSuccess) { cudaGetLastError(); return fail(B9_ENOMEM, "b9_drain_fetch: %llu bytes of re-push scratch: %s", (unsigned long long)c->res_in_bytes, cudaGetErrorString(e)); }
+        c->retry_bytes_cap = c->res_in_bytes;
+    }
+    size_t scan_bytes = 0;
+    CU(cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, c->d_in_off + 1, c->d_in_off + 1, (int)k, s));
+    if (c->retry_scan_cap < scan_bytes) {
+        cudaFree(c->d_retry_scan); c->d_retry_scan = nullptr; c->retry_scan_cap = 0;
+        const cudaError_t e = cudaMalloc(&c->d_retry_scan, scan_bytes);
+        if (e != cudaSuccess) { cudaGetLastError(); return fail(B9_ENOMEM, "b9_drain_fetch: re-push scan scratch: %s", cudaGetErrorString(e)); }
+        c->retry_scan_cap = scan_bytes;
+    }
+    const int64_t now = (int64_t)std::chrono::duration_cast<std::chrono::seconds>(std::chrono::system_clock::now().time_since_epoch()).count();
+    CU(cudaMemcpyAsync(c->d_retry_rec, retry_rec.data(), (size_t)k * 4, cudaMemcpyHostToDevice, s));
+    retry_len_kernel<<<(k + 255) / 256, 256, 0, s>>>(c->d_retry_rec, k, c->d_task_of, c->d_hdr, head, c->slot_mask, c->d_in_off);
+    CU(cudaGetLastError());
+    CU(cub::DeviceScan::InclusiveSum(c->d_retry_scan, scan_bytes, c->d_in_off + 1, c->d_in_off + 1, (int)k, s));
+    retry_gather_kernel<<<(uint32_t)(((uint64_t)k * 32 + 255) / 256), 256, 0, s>>>(c->d_retry_rec, k, c->d_task_of, head, c->slot_mask, c->d_payload,
+        c->d_off, c->d_hdr, c->d_ids, c->d_exp, c->d_in_off, now, c->d_retry_bytes, c->d_in_ts, c->d_in_exp, c->d_in_retries, c->d_in_flags, c->d_retry_ids);
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(&c->h_ctl->total, c->d_in_off + k, sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    const uint64_t bytes = c->h_ctl->total;
+    // Where the tasks go once the pop has released the window. The push segments the window consumes whole are free then;
+    // a segment it ends inside is trimmed to start at the first task behind the window (its offset is read back here), so
+    // that the window's bytes are free wherever they lie. The ring's free ranges then hold the retried bytes, which are at
+    // most the window's: they are placed in range order as one segment, or two when the freed bytes straddle the ring's end.
+    const uint64_t new_head = c->head_task + c->res_popped;               // (only drain-side calls move the head: out_mu is held)
+    Segment part{}; bool partial = false;
+    {
+        std::lock_guard<std::mutex> lk(c->mu);
+        for (const Segment& sg : c->segs)
+            if (sg.first_task < new_head && new_head < sg.first_task + sg.n) { part = sg; partial = true; break; }
+    }
+    uint64_t cut = 0;
+    if (partial) { const int rc = task_phys_off(c, part, new_head, &cut); if (rc) return rc; }
+    uint64_t reg[2][2]; int n_reg = 0; uint64_t wp = 0;
+    {
+        std::lock_guard<std::mutex> lk(c->mu);
+        bool have = false; uint64_t oldest = 0, live = 0;
+        for (const Segment& sg : c->segs) {
+            if (sg.first_task + sg.n <= new_head) continue;
+            const uint64_t st = (partial && sg.first_task == part.first_task) ? cut : sg.phys_start;
+            if (!have) { have = true; oldest = st; }
+            live += sg.bytes - (st - sg.phys_start);
+        }
+        wp = have ? c->write_pos : 0;
+        n_reg = b9_ring_free_ranges(c->ring_bytes, have, oldest, wp, live, reg);
+    }
+    // the plan: task range [i0, i1) at `at`, one entry per free range used (producers and drain-side calls are excluded
+    // until the commit below, so the ranges stay free)
+    struct Piece { uint32_t i0, i1; uint64_t at, end, lo, hi; };   // [lo, hi): its bytes in the scratch
+    Piece plan[2]; int n_plan = 0;
+    if (bytes == 0) plan[n_plan++] = Piece{0, k, wp, wp, 0, 0};                 // (empty HTTP bodies: no bytes to place)
+    else if (n_reg && bytes <= reg[0][1] - reg[0][0]) plan[n_plan++] = Piece{0, k, reg[0][0], reg[0][1], 0, bytes};
+    else if (n_reg == 2) {                                                 // split at a task boundary: the byte prefix is needed
+        std::vector<uint64_t> rel((size_t)k + 1);
+        CU(cudaMemcpyAsync(rel.data(), c->d_in_off, ((size_t)k + 1) * 8, cudaMemcpyDeviceToHost, s));
+        CU(cudaStreamSynchronize(s));
+        uint32_t i = 0;
+        for (int r = 0; r < 2 && i < k; ++r) {
+            const uint64_t room = reg[r][1] - reg[r][0];
+            const uint32_t e = (uint32_t)(std::upper_bound(rel.begin() + i, rel.end(), rel[i] + room) - rel.begin()) - 1u;
+            if (e > i) { plan[n_plan++] = Piece{i, e, reg[r][0], reg[r][1], rel[i], rel[e]}; i = e; }
+        }
+        if (i < k) n_plan = 0;
+    }
+    // (never taken: the retried tasks are at most the window's slots and bytes, and the pop frees both)
+    const bool slots_ok = (uint64_t)k <= (uint64_t)c->ring_tasks - (c->tail_task - new_head);
+    if (!slots_ok || n_plan == 0)
+        return fail(B9_ENOSPC, "b9_drain_fetch: the %u retried tasks (%llu bytes) find no room in the ring behind the pending ones; "
+                    "nothing is committed", k, (unsigned long long)bytes);
+    cudaEvent_t ready[2] = {nullptr, nullptr};
+    {
+        std::lock_guard<std::mutex> lk(c->mu);
+        for (int q = 0; q < n_plan && !c->event_pool.empty(); ++q) { ready[q] = c->event_pool.back(); c->event_pool.pop_back(); }
+    }
+    for (int q = 0; q < n_plan; ++q) if (!ready[q]) CU(cudaEventCreateWithFlags(&ready[q], cudaEventDisableTiming));
+    std::lock_guard<std::mutex> lk(c->mu);
+    c->stats.last_drain_d2h_ms = d2h_ms;
+    c->stats.bytes_d2h += c->res_bytes + (uint64_t)c->res_n * (16 + 1 + 1 + 8 + 4);
+    commit_pop(c);
+    if (partial)
+        for (Segment& sg : c->segs)
+            if (sg.first_task == part.first_task) {
+                sg.bytes -= cut - sg.phys_start; sg.n -= (uint32_t)(new_head - sg.first_task);
+                sg.first_task = new_head; sg.phys_start = cut;
+                break;
+            }
+    const uint64_t tail = c->tail_task;
+    // (enqueue only: nothing here waits for the device)
+    const uint32_t slot0 = (uint32_t)(tail & c->slot_mask);
+    const uint32_t first = std::min<uint32_t>(k, c->ring_tasks - slot0);
+    CU(cudaMemcpyAsync(c->d_ids + slot0, c->d_retry_ids, (size_t)first * 16, cudaMemcpyDeviceToDevice, s));
+    if (first < k) CU(cudaMemcpyAsync(c->d_ids, c->d_retry_ids + first, (size_t)(k - first) * 16, cudaMemcpyDeviceToDevice, s));
+    for (int q = 0; q < n_plan; ++q) {
+        const Piece& pc = plan[q];
+        const uint32_t n = pc.i1 - pc.i0;
+        if (pc.hi > pc.lo) CU(cudaMemcpyAsync(c->d_payload + pc.at, c->d_retry_bytes + pc.lo, pc.hi - pc.lo, cudaMemcpyDeviceToDevice, s));
+        ingest_kernel<<<(n + 255) / 256, 256, 0, s>>>(c->d_in_off + pc.i0, n, pc.at, tail + pc.i0, c->slot_mask, c->d_in_ts + pc.i0,
+                                                      c->d_in_exp + pc.i0, c->d_in_retries + pc.i0, c->d_in_flags + pc.i0,
+                                                      c->d_off, c->d_hdr, c->d_ts, c->d_exp);
+        CU(cudaGetLastError());
+        CU(cudaEventRecord(ready[q], s));
+        c->segs.push_back(Segment{tail + pc.i0, n, pc.at, pc.hi - pc.lo, ready[q], 0u});
+        c->write_pos = std::min<uint64_t>(pc.at + b9_seg_span(pc.hi - pc.lo), pc.end);
+    }
+    c->tail_task += k;
+    c->pending_bytes += bytes;
+    c->stats.kernel_launches += 3 + (uint64_t)n_plan;                      // (length, the scan, gather, ingest per segment)
+    return B9_OK;
+}
+
 }  // namespace
 
 extern "C" {
 
 uint32_t b9_abi_version(void) { return B9_ABI_VERSION; }
+
+int b9_set_retry_policy(b9_ctx* c, uint32_t exc_mask, uint32_t max_retries) {
+    if (!c) return fail(B9_EINVAL, "b9_set_retry_policy: ctx is NULL");
+    if (exc_mask & ~B9_EXC_ALL) return fail(B9_EINVAL, "b9_set_retry_policy: exception bits 0x%x are not B9_EXC_*", exc_mask & ~B9_EXC_ALL);
+    if (max_retries > 255) return fail(B9_EINVAL, "b9_set_retry_policy: max_retries %u: a task's retries are one byte (b9_push_meta.retries)", max_retries);
+    OutLock out_lk(c);
+    if (exc_mask && !c->d_task_of) {
+        CU(cudaSetDevice(c->device));
+        const size_t md = c->max_drain_tasks;
+        cudaError_t e = cudaMalloc(&c->d_task_of, md * sizeof(uint32_t));
+        if (e == cudaSuccess) e = cudaMalloc(&c->d_retry_rec, md * sizeof(uint32_t));
+        if (e == cudaSuccess) e = cudaMalloc(&c->d_retry_ids, md * sizeof(uint4));
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            cudaFree(c->d_task_of); cudaFree(c->d_retry_rec); cudaFree(c->d_retry_ids);
+            c->d_task_of = nullptr; c->d_retry_rec = nullptr; c->d_retry_ids = nullptr;
+            return fail(e == cudaErrorMemoryAllocation ? B9_ENOMEM : B9_EIO, "b9_set_retry_policy: %s", cudaGetErrorString(e));
+        }
+    }
+    c->retry_mask = exc_mask;
+    c->max_retries = max_retries;
+    return B9_OK;
+}
 
 int b9_device_count(void) {
     int n = 0;
@@ -510,6 +703,7 @@ void b9_ctx_destroy(b9_ctx* c) {
     cudaFree(c->d_out_payload); cudaFree(c->d_out_off); cudaFree(c->d_out_ids); cudaFree(c->d_out_status); cudaFree(c->d_out_has); cudaFree(c->d_out_len); cudaFree(c->d_slow); cudaFree(c->d_wire_env); cudaFree(c->d_crc_shift);
     cudaFree(c->d_ctl); cudaFree(c->d_tile_state); cudaFree(c->d_count);
     cudaFree(c->d_cancel_keys); cudaFree(c->d_cancel_out);
+    cudaFree(c->d_task_of); cudaFree(c->d_retry_rec); cudaFree(c->d_retry_ids); cudaFree(c->d_retry_bytes); cudaFree(c->d_retry_scan);
     if (c->h_ctl) cudaFreeHost(c->h_ctl);
     if (c->h_rtab) cudaFreeHost(c->h_rtab);
     cudaFree(c->d_rtab); cudaFree(c->d_prefix); cudaFree(c->d_scan_sums);
@@ -948,6 +1142,7 @@ static int64_t drain_launch_common(b9_ctx* c, int handler, uint32_t max_tasks, i
     c->have_results = false; c->res_async = false;
     c->running.store(0, std::memory_order_relaxed);
     c->res_n = 0; c->res_popped = 0; c->res_bytes = 0; c->res_in_bytes = 0; c->res_peek = (peek & B9_DRAIN_PEEK) != 0;
+    c->res_gen++; c->res_retry = false;
     cudaStream_t s = c->stream;
     // the window: a snapshot of the ring's head under the bookkeeping lock. Only drain-side calls (all under out_mu)
     // move the head or free segments, so the snapshot stays valid while the launch is prepared without c->mu.
@@ -990,6 +1185,8 @@ static int64_t drain_launch_common(b9_ctx* c, int handler, uint32_t max_tasks, i
     a.count_mode = count_mode;
     a.slow = c->d_slow; a.crc_shift_tabs = c->d_crc_shift;
     a.static_rounds = 0;
+    a.retry_mask = endpoint ? 0u : c->retry_mask; a.max_retries = c->max_retries; a.task_of = c->d_task_of;
+    c->res_retry = a.retry_mask != 0;
     c->drain_epoch = (c->drain_epoch + 1u) & 0xFFFFFFu;
     if (c->drain_epoch == 0u) {                                             // the 24-bit tag wrapped: forget old tags
         c->drain_epoch = 1u; c->ctl_dirty = true;                           // (and the control ring's order)
@@ -1076,7 +1273,9 @@ int64_t b9_endpoint_drain_launch(b9_ctx* c, int handler, uint32_t max_tasks, int
 
 int64_t b9_drain_fetch(b9_ctx* c, b9_results* out) {
     if (!c || !out) return fail(B9_EINVAL, "b9_drain_fetch: NULL argument");
-    OutLock out_lk(c);
+    std::unique_lock<std::mutex> in_lk(c->in_mu, std::defer_lock);
+    std::unique_lock<std::mutex> out_lk(c->out_mu);
+    end_drain_span(c);
     CU(cudaSetDevice(c->device));
     { int rc = finish_launch(c); if (rc) return rc; }
     if (!c->have_results) return fail(B9_EINVAL, "b9_drain_fetch: no drain results are waiting");
@@ -1108,24 +1307,37 @@ int64_t b9_drain_fetch(b9_ctx* c, b9_results* out) {
     CU(cudaEventRecord(c->ev_d, s));
     CU(cudaStreamSynchronize(s));
     float ms = 0; cudaEventElapsedTime(&ms, c->ev_c, c->ev_d);
+    // the window's RETRY records (only a drain under a retry policy writes them), in record order: pushed again below
+    std::vector<uint32_t> retry_rec;
+    if (!c->res_peek && c->res_retry)
+        for (size_t j = 0; j < n; ++j) if (out->status[j] == B9_ST_RETRY) retry_rec.push_back((uint32_t)j);
     // TaskQueueCompleteRequest.task_duration (taskqueue.proto:50): the runner reports the seconds it spent on a task; a
     // drain spends kernel + read-back time on res_popped tasks at once, so every task of the batch is charged its share
     if (c->res_popped) out->task_duration = (c->res_kernel_ms + ms) * 1e-3f / (float)c->res_popped;
-    {
+    if (!retry_rec.empty()) {
+        // the re-push is a push: it takes the producers' lock, so that concurrent pushes land wholly before or after it. The
+        // lock order is in_mu before out_mu: when a producer holds in_mu, out_mu is let go while the fetch waits for it, and
+        // the commit goes ahead only if no other drain-side call has touched these results meanwhile
+        if (!in_lk.try_lock()) {
+            const uint64_t gen = c->res_gen;
+            out_lk.unlock();
+            in_lk.lock();
+            out_lk.lock();
+            end_drain_span(c);
+            if (c->res_gen != gen || !c->have_results)
+                return fail(B9_EINVAL, "b9_drain_fetch: another drain-side call replaced or committed these results meanwhile");
+        }
+        const int rc = commit_with_repush(c, retry_rec, ms);
+        if (rc) return rc;
+    } else {
         std::lock_guard<std::mutex> lk(c->mu);
         c->stats.last_drain_d2h_ms = ms;
         c->stats.bytes_d2h += c->res_bytes + n * (16 + 1 + 1 + 8 + 4);
-        if (!c->res_peek) {
-            c->head_task += c->res_popped; c->pending_bytes -= c->res_in_bytes; c->stats.tasks_drained += c->res_popped;
-            c->cancelled_pending -= std::min<uint64_t>(c->cancelled_pending, (uint64_t)(c->res_popped - c->res_n));
-            c->recount_cancelled = c->expired_since_launch;              // an expire ran between this drain's launch and its commit: its
-                                                                          // count included tasks of the window that are gone now
-            free_segments(c);
-        }
+        if (!c->res_peek) commit_pop(c);
     }
     if (!c->res_peek && c->recount_cancelled) { int rc = recount_cancelled_locked_out(c); if (rc) return rc; }
     c->running.store(0, std::memory_order_relaxed);
-    c->have_results = false; c->res_async = false; c->burst_open = false;
+    c->have_results = false; c->res_async = false; c->burst_open = false; c->res_gen++;
     return (int64_t)n;
 }
 
@@ -1182,6 +1394,7 @@ static int64_t wire_encode(b9_ctx* c, const b9_wire_env* env, uint32_t max_tasks
         for (const Segment& sg : c->segs) CU(cudaStreamWaitEvent(s, sg.ready, 0));
     }
     c->res_n = 0; c->res_popped = 0; c->res_bytes = 0; c->res_in_bytes = 0; c->res_peek = true;
+    c->res_gen++; c->res_retry = false;
     if (n == 0) { c->have_results = true; return 0; }
     WireEnv we; memset(&we, 0, sizeof we);
     {

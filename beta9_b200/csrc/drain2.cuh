@@ -1311,7 +1311,7 @@ __device__ __noinline__ void slow_task(const DrainArgs& a, uint64_t goff, uint32
         else if (rec.mode == OM_COPY) warp_copy(o, p + rec.src_off, rec.src_len, lane);
         else if (lane == 0) seq_emit<true>(p, rec, o);
     }
-    if (lane == 0) store_record(a.out, j, r.fits, r.base, rec.out_len, rec.status, rec.has);
+    if (lane == 0) store_record(a.out, j, r.fits, r.base, rec.out_len, retry_settle(a, j, ~0u, rec.status, rec.value), rec.has);
     __syncwarp();
 }
 
@@ -1354,7 +1354,8 @@ __device__ __noinline__ void d3_identity_tail(const DrainArgs& a, uint8_t* __res
     }
 }
 
-template <int HANDLER>
+// RETRY: the context has a retry policy (DrainArgs::retry_mask); without one the kernel is the same as before the policy existed
+template <int HANDLER, bool RETRY>
 __global__ void __launch_bounds__(D3_WARPS * 32, D3Cfg<HANDLER>::MIN_BLOCKS) drain3_kernel(DrainArgs a, uint32_t in_cap, uint32_t warp_stride) {
     constexpr int T = D3Cfg<HANDLER>::T;
     const uint32_t TT = (HANDLER == 3) ? a.tile_tasks : (uint32_t)T;      // tasks per tile: json_sum's is chosen per launch (<= T)
@@ -1611,9 +1612,10 @@ __global__ void __launch_bounds__(D3_WARPS * 32, D3Cfg<HANDLER>::MIN_BLOCKS) dra
                 SlowItem* it = a.slow + atomicAdd(&a.out.ctl->n_slow, 1u);
                 it->w1 = (unsigned long long)(my_len | (rec.value == 1 ? 0x80000000u : 0u) | (my_http ? 0x40000000u : 0u)) | ((unsigned long long)j << 32) | (rec.value == 2 ? (1ull << 56) : 0ull)
                        | (rec.value == 3 ? (1ull << 57) : 0ull);
+                if (RETRY) a.task_of[j] = t0 + lane;                       // (the tail's retry_settle looks the task up)
                 __threadfence();
                 *(volatile unsigned long long*)&it->w0 = my_goff | ((unsigned long long)a.epoch << 40);
-            } else store_record(a.out, j, fits, ob, rec.out_len, rec.status, rec.has);
+            } else store_record(a.out, j, fits, ob, rec.out_len, RETRY ? retry_settle(a, j, t0 + lane, rec.status, rec.value) : rec.status, rec.has);
             if (rec.has && fits) {
                 if (rec.mode == OM_COPY) {
                     if (coal) {}                                            // written by d3_copy_tile

@@ -18,6 +18,7 @@ __host__ __device__ __forceinline__ uint64_t hdr_pack(uint32_t len, uint8_t flag
 }
 __host__ __device__ __forceinline__ uint32_t hdr_len(uint64_t h) { return (uint32_t)h; }
 __host__ __device__ __forceinline__ uint32_t hdr_flags(uint64_t h) { return (uint32_t)(h >> 32) & 0xFFu; }
+__host__ __device__ __forceinline__ uint32_t hdr_retries(uint64_t h) { return (uint32_t)(h >> 40) & 0xFFu; }
 constexpr uint32_t B9_TF_HTTP_BODY_BIT = 0x02u;      // == B9_TF_HTTP_BODY (include/b9gpu.h)
 constexpr uint32_t B9_TF_PICKLE_BIT    = 0x04u;      // == B9_TF_PICKLE
 constexpr uint32_t B9_TF_TASK_MSG_BIT  = 0x08u;      // == B9_TF_TASK_MSG
@@ -128,7 +129,25 @@ struct DrainArgs {
     const uint32_t* crc_shift_tabs; // crc32: [levels][4][256] "advance the CRC register over 2^k zero bytes" tables
     uint32_t static_rounds;         // a worker's first static_rounds tiles are worker + q * workers, the rest come from the ticket counter
     uint32_t tile_tasks;            // json_sum: tasks per warp-tile of THIS launch (4 or 8: small windows balance better on finer tiles); others: fixed
+    // the context's retry policy (b9_set_retry_policy): an ERROR whose class is in retry_mask is RETRY / RETRY_LIMIT
+    uint32_t retry_mask;            // B9_EXC_* bits; 0 = no policy: every answer as without one
+    uint32_t max_retries;
+    uint32_t* task_of;              // [n_tasks] with a policy: the window task of record j, written for RETRY records (b9_drain_fetch
+                                    // re-pushes them) and, by identity's main loop, for every task it defers to the kernel's tail
+                                    // (drain3_kernel<H, true>: the launch with a policy; <H, false> is the drain without one)
 };
+
+// The status record j (of window task t) is written with: an ERROR whose exception class the retry policy names becomes
+// RETRY while the task's retries are below max_retries, else RETRY_LIMIT (Dispatcher.RetryTask's test,
+// pkg/task/dispatch.go:232-285). `value` is rec.value: an ERROR's exception class. t == ~0u: task_of[j] holds the task.
+__device__ __forceinline__ uint8_t retry_settle(const DrainArgs& a, uint32_t j, uint32_t t, uint8_t status, long long value) {
+    if (status != ST_ERROR || !((uint32_t)value & a.retry_mask)) return status;
+    if (t == ~0u) t = a.task_of[j];
+    const uint32_t retries = hdr_retries(__ldg(a.hdr + (uint32_t)((a.first_task + t) & a.slot_mask)));
+    if (retries >= a.max_retries) return (uint8_t)ST_RETRY_LIMIT;
+    a.task_of[j] = t;
+    return (uint8_t)ST_RETRY;
+}
 
 // where record j's id is, once store_record_id has run for it (DrainOut::ids_compacted)
 __device__ __forceinline__ const uint4* record_id(const DrainArgs& a, uint32_t j) {

@@ -22,8 +22,20 @@ struct TaskRec {
     uint32_t src_len;
     uint32_t out_len;
     uint8_t  status, has, mode, ready;
-    long long value;     // OM_U32_DEC / OM_I64_DEC; the float64's bits for OM_PY_NUM / OM_PY_FLOAT
+    long long value;     // OM_U32_DEC / OM_I64_DEC; the float64's bits for OM_PY_NUM / OM_PY_FLOAT; status ERROR: the
+                         // exception class the handler raised (one EXC_* bit), for the retry policy (retry_settle)
 };
+
+// the exception classes of include/b9gpu.h's B9_EXC_* (the retry policy matches them exactly, as retry_on_errors does)
+constexpr uint8_t EXC_TYPE = 0x01, EXC_ATTRIBUTE = 0x02, EXC_UNICODE_ENCODE = 0x04, EXC_KEY = 0x08, EXC_VALUE = 0x10, EXC_BINASCII = 0x20;
+
+// base64.b64decode(s, validate=True) of a str that is not valid base64: `s.encode('ascii')` comes first, so a non-ASCII
+// character anywhere is ValueError, otherwise binascii.Error. p[s..e) is the validated string token, quotes included.
+__device__ inline uint8_t b64_str_error_class(const uint8_t* __restrict__ p, uint32_t s, uint32_t e) {
+    uint32_t i = s + 1;
+    while (i < e - 1) if (next_cp(p, i, e - 1) >= 0x80) return EXC_VALUE;
+    return EXC_BINASCII;
+}
 
 // String token p[s..e) (quotes included, validated): does the Python-escaped form equal a plain
 // copy?  Computes the json.dumps length either way. One thread.
@@ -174,7 +186,7 @@ __device__ inline void handler_phase_a(int handler, const uint8_t* __restrict__ 
     rec.has = 0; rec.mode = OM_NONE; rec.out_len = 0; rec.src_off = 0; rec.src_len = 0; rec.value = 0;
     if (pr.status != ST_OK) { rec.status = pr.status; return; }
     // handler(*args, **kwargs) with a positional-only one-parameter handler
-    if (pr.nargs != 1 || pr.kwargs_nonempty) { rec.status = 1 /* ERROR: TypeError */; return; }
+    if (pr.nargs != 1 || pr.kwargs_nonempty) { rec.status = ST_ERROR; rec.value = EXC_TYPE; return; }
     rec.status = 0;
     switch (handler) {
     case 0: {   // identity: result = args[0]; `serialize_result(result) if result else None`
@@ -212,34 +224,42 @@ __device__ inline void handler_phase_a(int handler, const uint8_t* __restrict__ 
         }
     }
     case 1: {   // crc32: zlib.crc32(s.encode()); a non-str has no .encode -> AttributeError
-        if (pr.a0_kind != AK_STR) { rec.status = 1; return; }
+        if (pr.a0_kind != AK_STR) { rec.status = ST_ERROR; rec.value = EXC_ATTRIBUTE; return; }
         uint32_t c = crc32_of_string_token(p, pr.a0_off, pr.a0_off + pr.a0_len, pr.a0_flags, crc_table);
         if (c == 0) return;                                                 // 0 is falsy
         rec.value = (long long)c; rec.out_len = dec_len_u64(c); rec.mode = OM_U32_DEC; rec.has = 1;
         return;
     }
     case 2: {   // vadd_f32: base64 -> fp32 a||b -> a+b -> base64
-        if (pr.a0_kind != AK_STR) { rec.status = 1; return; }               // TypeError
-        if (pr.a0_flags & SF_NONPRINT) { rec.status = 1; return; }          // non-ASCII / DEL: ValueError / binascii.Error
+        if (pr.a0_kind != AK_STR) { rec.status = ST_ERROR; rec.value = EXC_TYPE; return; }
+        if (pr.a0_flags & SF_NONPRINT) {                                    // non-ASCII / DEL: ValueError / binascii.Error
+            rec.status = ST_ERROR; rec.value = b64_str_error_class(p, pr.a0_off, pr.a0_off + pr.a0_len); return;
+        }
         if (pr.a0_flags & SF_ESC) {
             // escaped text: any decoded character outside the base64 alphabet is an error for sure;
             // a fully valid escaped base64 string (only "\/" can do that) is not produced by the SDK
             uint32_t i = pr.a0_off + 1, end = pr.a0_off + pr.a0_len - 1;
-            while (i < end) { uint32_t cp = next_cp(p, i, end); if (cp >= 0x80 || (b64_val((uint8_t)cp) < 0 && cp != '=')) { rec.status = 1; return; } }
+            while (i < end) {
+                uint32_t cp = next_cp(p, i, end);
+                if (cp >= 0x80 || (b64_val((uint8_t)cp) < 0 && cp != '=')) {
+                    rec.status = ST_ERROR; rec.value = b64_str_error_class(p, pr.a0_off, pr.a0_off + pr.a0_len); return;
+                }
+            }
             rec.status = ST_UNSUPPORTED; return;
         }
         int64_t rn = b64_decoded_len(p, pr.a0_off + 1, pr.a0_off + pr.a0_len - 1);
-        if (rn < 0 || (rn % 8)) { rec.status = 1; return; }
+        if (rn < 0 || (rn % 8)) { rec.status = ST_ERROR; rec.value = rn < 0 ? EXC_BINASCII : EXC_VALUE; return; }
         uint32_t n = (uint32_t)(rn / 8);
         if (n == 0) return;                                                 // "" is falsy
         rec.src_off = pr.a0_off + 1; rec.src_len = n; rec.out_len = 2 + b64_encoded_len(4 * n); rec.mode = OM_VADD; rec.has = 1;
         return;
     }
     case 3: {   // json_sum: sum(obj["values"])
-        if (pr.a0_kind != AK_OBJ) { rec.status = 1; return; }               // TypeError, or KeyError for {}
+        if (pr.a0_kind != AK_OBJ) { rec.status = ST_ERROR; rec.value = pr.a0_kind == AK_OBJ_EMPTY ? EXC_KEY : EXC_TYPE; return; }
         PySum ps;
-        int st = json_sum_object(p, pr.a0_off, pr.a0_off + pr.a0_len, &ps);
-        if (st) { rec.status = (uint8_t)st; return; }
+        bool no_key = false;
+        int st = json_sum_object(p, pr.a0_off, pr.a0_off + pr.a0_len, &ps, &no_key);
+        if (st) { rec.status = (uint8_t)st; if (st == ST_ERROR) rec.value = no_key ? EXC_KEY : EXC_TYPE; return; }
         if (ps.is_float) {                                                  // 0.0 / -0.0 are falsy, NaN is not
             const unsigned long long b = f64_to_bits(ps.f);
             if ((b << 1) == 0) return;

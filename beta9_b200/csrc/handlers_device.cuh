@@ -159,7 +159,8 @@ __device__ __noinline__ int sum_values_token(const uint8_t* __restrict__ p, uint
 }
 
 // arg token p[s..e) is a non-empty object (validated). Finds the last "values" key.
-__device__ inline int json_sum_object(const uint8_t* __restrict__ p, uint32_t s, uint32_t e, PySum* sum) {
+// *no_key (optional): set when the status is ERROR because there is no "values" (KeyError rather than TypeError)
+__device__ inline int json_sum_object(const uint8_t* __restrict__ p, uint32_t s, uint32_t e, PySum* sum, bool* no_key = nullptr) {
     uint32_t i = s + 1;
     bool found = false; uint32_t vs = 0, ve = 0;
     for (;;) {
@@ -178,7 +179,7 @@ __device__ inline int json_sum_object(const uint8_t* __restrict__ p, uint32_t s,
         if (p[i] == ',') { ++i; continue; }
         break;                                                     // '}'
     }
-    if (!found) return 1;                                          // KeyError
+    if (!found) { if (no_key) *no_key = true; return 1; }          // KeyError
     return sum_values_token(p, vs, ve, sum);
 }
 

@@ -29,7 +29,7 @@ constexpr uint32_t SF_NUM_EXP  = 1u << 2;  // a number with exponent or > 300 di
 constexpr uint32_t SF_DEEP     = 1u << 3;  // nesting deeper than the device stack
 constexpr uint32_t SF_F64_OVER = 1u << 4;  // a number literal that strconv.ParseFloat rejects with ErrRange
 
-constexpr int ST_OK = 0, ST_REJECTED = 3, ST_UNSUPPORTED = 4;
+constexpr int ST_OK = 0, ST_ERROR = 1, ST_RETRY = 2, ST_REJECTED = 3, ST_UNSUPPORTED = 4, ST_RETRY_LIMIT = 5;   // == enum b9_status
 
 struct Parsed {
     uint8_t  status;          // ST_OK / ST_REJECTED / ST_UNSUPPORTED

@@ -29,7 +29,6 @@ constexpr uint32_t PK_MAX_DEPTH  = 16;      // identity: containers nested in a 
 constexpr uint32_t PK_MAX_MEMBERS = 64;     // members of one dict (PY_VALUE_MAX_MEMBERS of the JSON path)
 constexpr uint32_t PK_FRAME_TARGET = 65536; // the pickler's FRAME_SIZE_TARGET: a result body this long is declined
 constexpr uint16_t PK_NIL = 0xFFFFu;
-constexpr int ST_ERROR = 1;                 // (B9_ST_ERROR: the handler raised)
 
 enum : uint8_t { PK_NONE, PK_FALSE, PK_TRUE, PK_INT, PK_FLOAT, PK_STR, PK_BYTES, PK_LIST, PK_TUPLE, PK_DICT };
 

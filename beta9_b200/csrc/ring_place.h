@@ -38,3 +38,22 @@ static inline int b9_ring_place(uint64_t ring_bytes, int have_segments, uint64_t
     if (wp + need <= oldest) { *start = wp; return 1; }  // wrapped already: free is [wp, oldest)
     return 0;
 }
+
+// The free byte ranges of the same model, in the order b9_ring_place tries them: reg[i] = [start, end). Returns their
+// number (0, 1 or 2). A segment may fill a range exactly; the next free byte after it is then min(its start +
+// b9_seg_span(bytes), the range's end) — the re-push of retried tasks places its segments this way, so that tasks whose
+// bytes were exactly the window's fit back into a ring that was exactly full.
+static inline int b9_ring_free_ranges(uint64_t ring_bytes, int have_segments, uint64_t oldest, uint64_t wp, uint64_t live_bytes,
+                                      uint64_t reg[2][2]) {
+    if (!have_segments) { reg[0][0] = 0; reg[0][1] = ring_bytes; return 1; }
+    if (live_bytes == 0) { reg[0][0] = 0; reg[0][1] = ring_bytes; return 1; }   // positions carry no data
+    if (wp == oldest) return 0;
+    if (wp > oldest) {
+        int n = 0;
+        if (wp < ring_bytes) { reg[n][0] = wp; reg[n][1] = ring_bytes; ++n; }
+        if (oldest > 0) { reg[n][0] = 0; reg[n][1] = oldest; ++n; }
+        return n;
+    }
+    reg[0][0] = wp; reg[0][1] = oldest;
+    return 1;
+}

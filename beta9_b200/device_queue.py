@@ -6,9 +6,10 @@ All buffers are numpy arrays; results come back packed (see `DrainResult`).
 """
 from __future__ import annotations
 
+import binascii
 import ctypes as C
 from dataclasses import dataclass
-from typing import List, Optional, Tuple
+from typing import Iterable, List, Optional, Tuple
 
 import numpy as np
 
@@ -17,7 +18,22 @@ from . import _lib as L
 HANDLERS = {"identity": L.H_IDENTITY, "echo": L.H_IDENTITY, "crc32": L.H_CRC32,
             "vadd_f32": L.H_VADD_F32, "json_sum": L.H_JSON_SUM}
 STATUS_NAMES = {L.ST_COMPLETE: "COMPLETE", L.ST_ERROR: "ERROR", L.ST_RETRY: "RETRY",
-                L.ST_REJECTED: "REJECTED", L.ST_UNSUPPORTED: "UNSUPPORTED"}
+                L.ST_REJECTED: "REJECTED", L.ST_UNSUPPORTED: "UNSUPPORTED", L.ST_RETRY_LIMIT: "RETRY_LIMIT"}
+# every exception class a device handler can raise, and its B9_EXC_* bit (include/b9gpu.h)
+EXC_BITS = {TypeError: L.EXC_TYPE_ERROR, AttributeError: L.EXC_ATTRIBUTE_ERROR, UnicodeEncodeError: L.EXC_UNICODE_ENCODE,
+            KeyError: L.EXC_KEY_ERROR, ValueError: L.EXC_VALUE_ERROR, binascii.Error: L.EXC_BINASCII_ERROR}
+
+
+def retry_mask(retry_for: Optional[Iterable[type]]) -> int:
+    """The B9_EXC_* bits of a `retry_for` list. The runner retries on `type(e) is err` (retry_on_errors, an exact match),
+    so classes map by identity: a subclass or a class outside EXC_BITS is never what a device handler raises, and adds
+    nothing."""
+    m = 0
+    for err in retry_for or ():
+        for cls, bit in EXC_BITS.items():
+            if err is cls:
+                m |= bit
+    return m
 
 
 @dataclass
@@ -170,6 +186,13 @@ class DeviceQueue:
         outcome = np.zeros(max(n, 1), np.uint8)
         marked = self._check(self._lib.b9_cancel(self._ctx, ids.ctypes.data if n else None, n, outcome.ctypes.data))
         return marked, outcome[:n]
+
+    def set_retry_policy(self, retry_for: Optional[Iterable[type]], max_retries: int) -> None:
+        """b9_set_retry_policy: the stub's `retry_for` classes and TaskPolicy.MaxRetries. A task whose handler raised one of
+        them comes back RETRY (and is pushed again, retries + 1, when its drain is fetched) or, once its retries reached
+        max_retries, RETRY_LIMIT. An empty `retry_for` restores the answers without a policy. max_retries is at most 255
+        (a task's retries are one byte); a larger value raises B9Error (B9_EINVAL)."""
+        self._check(self._lib.b9_set_retry_policy(self._ctx, retry_mask(retry_for), max(0, int(max_retries))))
 
     # ---- consumer side
     def drain(self, handler: str, max_tasks: int = 1 << 22, cap_bytes: Optional[int] = None, full_pickle: bool = False,

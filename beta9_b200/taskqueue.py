@@ -42,18 +42,21 @@ class Task:
 
 class TaskQueue:
     """Decorator. Resource arguments are accepted and kept for API compatibility; only the ones
-    this path reads have an effect (`max_pending_tasks`, `gpu_handler`, `device`)."""
+    this path reads have an effect (`max_pending_tasks`, `retries`, `retry_for`, `gpu_handler`, `device`). A task whose
+    handler raises a class in `retry_for` (an exact match, as the runner's retry_on_errors) comes back "RETRY" and is
+    queued again, up to `retries` times; after that it comes back "RETRY_LIMIT" (the gateway cancels it)."""
 
     def __init__(self, cpu: Union[int, float, str] = 1.0, memory: Union[int, str] = 128, gpu: Any = "", image: Any = None,
                  timeout: int = 3600, retries: int = 3, workers: int = 1, keep_warm_seconds: int = 10,
                  max_pending_tasks: int = DEFAULT_MAX_PENDING_TASKS, name: Optional[str] = None,
-                 gpu_handler: Optional[str] = None, device: int = 0, queue: Optional[DeviceQueue] = None, **kwargs: Any):
+                 retry_for: Optional[List[type]] = None, gpu_handler: Optional[str] = None, device: int = 0, queue: Optional[DeviceQueue] = None, **kwargs: Any):
         self.cpu = int(float(cpu) * 1000) if not isinstance(cpu, str) else cpu     # base/runner.py parse_cpu: cores -> millicores
         self.memory = memory
         self.gpu = gpu
         self.image = image
         self.timeout = timeout
         self.retries = retries
+        self.retry_for = list(retry_for or [])
         self.workers = workers
         self.keep_warm_seconds = keep_warm_seconds
         self.max_pending_tasks = max_pending_tasks
@@ -62,12 +65,16 @@ class TaskQueue:
         self.device = device
         self.extra = kwargs
         self._queue = queue
+        self._policy_set = False
         self.stub_id = str(uuid.uuid4())
 
     @property
     def queue(self) -> DeviceQueue:
         if self._queue is None:
             self._queue = DeviceQueue(device=self.device)     # raises without a GPU: no CPU path
+        if not self._policy_set:
+            self._queue.set_retry_policy(self.retry_for, self.retries)
+            self._policy_set = True
         return self._queue
 
     def prepare_runtime(self, func: Optional[Callable] = None, stub_type: str = TASKQUEUE_STUB_TYPE) -> bool:
@@ -206,7 +213,8 @@ class _CallableWrapper:
                 break                                         # cancelled / expired tasks produce no record: their result is None
             for t in got:
                 if t.id in want:
-                    done[t.id] = t
+                    if t.status != "RETRY":                   # a retried task is queued again: its answer comes later
+                        done[t.id] = t
                 else:
                     self._held.append(t)
         for t in tasks:

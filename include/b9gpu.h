@@ -80,8 +80,28 @@ enum b9_status {
     B9_ST_ERROR       = 1,
     B9_ST_RETRY       = 2,
     B9_ST_REJECTED    = 3,
-    B9_ST_UNSUPPORTED = 4
+    B9_ST_UNSUPPORTED = 4,
+    /* The runner reported Retry (see b9_set_retry_policy), but the task's Retries had reached Policy.MaxRetries: the
+     * gateway cancels it with TaskExceededRetryLimit and completes it instead of re-queueing it
+     * (pkg/abstractions/taskqueue/taskqueue.go:680-710, pkg/task/dispatch.go:232-285). has_result = 0. */
+    B9_ST_RETRY_LIMIT = 5
 };
+
+/* ---- the exception class a device handler raises, for b9_set_retry_policy --------------------------------------
+ * The runner answers TaskStatus.Retry instead of Error when `type(e) is err` for an `err` in the stub's `retry_for`
+ * (sdk/src/beta9/runner/taskqueue.py:352-393,407-408): an exact class match, so B9_EXC_VALUE_ERROR does not
+ * cover binascii.Error. The classes the four handlers (oracle/pyoracle/handlers.py) can raise on CPython 3.12:   */
+#define B9_EXC_TYPE_ERROR       0x01u  /* any handler: not exactly one positional argument, or keyword arguments; vadd_f32 of a
+                                          non-str; json_sum of a non-dict, of a "values" that is not iterable or holds a
+                                          non-number (a dict "values" sums its str keys)                                     */
+#define B9_EXC_ATTRIBUTE_ERROR  0x02u  /* crc32 of a non-str (no .encode)                                                    */
+#define B9_EXC_UNICODE_ENCODE   0x04u  /* crc32 of a str holding a lone surrogate. Never raised on the device: Go's decoder
+                                          replaces lone surrogates with U+FFFD, and TASK_MSG records holding one are declined */
+#define B9_EXC_KEY_ERROR        0x08u  /* json_sum of a dict without "values"                                                 */
+#define B9_EXC_VALUE_ERROR      0x10u  /* vadd_f32 of a str with a non-ASCII character, or whose decoded length is not a
+                                          multiple of 8                                                                      */
+#define B9_EXC_BINASCII_ERROR   0x20u  /* vadd_f32 of an ASCII str that is not base64 under validate=True (binascii.Error)    */
+#define B9_EXC_ALL              0x3Fu
 
 /* ---- per-task flags (b9_push_meta.flags / ring header) ------------------------------------ */
 #define B9_TF_CANCELLED 0x01u  /* task already completed/cancelled/expired: TaskQueuePop skips it
@@ -282,6 +302,22 @@ int64_t  b9_expire(b9_ctx *ctx, int64_t now_unix_ns);
 #define B9_CANCEL_CLAIMED  0x04u  /* a task with this id is in the window of an outstanding drain: left alone, its record
                                      comes back with that drain's b9_drain_fetch                                        */
 int64_t  b9_cancel(b9_ctx *ctx, const uint8_t *task_ids, uint32_t n, uint8_t *outcome);
+
+/* The stub's retry policy: `retry_for` as B9_EXC_* bits and TaskPolicy.MaxRetries (pkg/types/task.go:118-123). One ctx is
+ * one stub's queue, so the policy belongs to the ctx; it applies to the b9_drain_launch calls made after it (a drain-side
+ * call). exc_mask 0, the default, keeps every answer as it is without a policy. With a mask, a task-queue task whose
+ * handler raised a class in the mask gets, instead of B9_ST_ERROR, B9_ST_RETRY while its retries (b9_push_meta.retries)
+ * are below max_retries and B9_ST_RETRY_LIMIT after; has_result = 0 in both. When b9_drain_fetch / b9_drain_fetch_object
+ * commits the pop, every RETRY task is pushed again at the tail of the ring in record order, on the device (the RPUSH of
+ * Dispatcher.RetryTask, pkg/task/dispatch.go:232-285): same id, payload bytes, flags and expiry, retries + 1, timestamp =
+ * the host clock at the commit. That re-push is a push: it waits for a producer's push in progress, concurrent pushes land
+ * wholly before or after it, and it counts in b9_depth. It always finds room, also in a ring that was exactly full: its
+ * slots are at most the window's, and its bytes at most the window's, which the commit frees wherever they lie (a push
+ * segment the window ends inside is trimmed to its unconsumed tasks; DESIGN.md §4.9). Not affected: B9_TF_PICKLE tasks, b9_endpoint_drain_launch, and
+ * B9_DRAIN_PEEK launches (their records show RETRY / RETRY_LIMIT, but nothing is popped or pushed). Returns 0, or B9_EINVAL
+ * for a NULL ctx, bits outside B9_EXC_ALL, or max_retries above 255 (a slot's retries is one byte, as b9_push_meta.retries).
+ * Added without an ABI version change: probe for it with dlsym. */
+int      b9_set_retry_policy(b9_ctx *ctx, uint32_t exc_mask, uint32_t max_retries);
 
 /* ---- consumer side ---------------------------------------------------------------------------
  * b9_drain replaces, for up to max_tasks pending tasks in FIFO order, the whole
