@@ -17,6 +17,7 @@ TF_CANCELLED = 0x01
 TF_HTTP_BODY, TF_PICKLE, TF_TASK_MSG = 0x02, 0x04, 0x08
 CANCEL_MARKED, CANCEL_ALREADY, CANCEL_CLAIMED = 0x01, 0x02, 0x04      # b9_cancel outcome bits
 DRAIN_PEEK, DRAIN_ASYNC, DRAIN_PICKLE_FULL = 1, 2, 4                   # b9_drain_launch flags
+CB_NONE, CB_POST, CB_UNSENDABLE, CB_HOST = 0, 1, 2, 3                  # enum b9_callback_kind
 
 
 class Opts(C.Structure):
@@ -35,6 +36,10 @@ class Results(C.Structure):
                 ("offsets", C.c_void_p), ("lengths", C.c_void_p), ("payload", C.c_void_p), ("cap_tasks", C.c_uint32),
                 ("cap_bytes", C.c_uint64), ("n_results", C.c_uint32), ("n_popped", C.c_uint32),
                 ("n_bytes", C.c_uint64), ("need_bytes", C.c_uint64), ("task_duration", C.c_float), ("reserved_", C.c_uint32)]
+
+
+class Callbacks(C.Structure):
+    _fields_ = [("kind", C.c_void_p), ("digest", C.c_void_p), ("cap_tasks", C.c_uint32), ("timestamp", C.c_int64)]
 
 
 class Stats(C.Structure):
@@ -84,6 +89,8 @@ SYMBOLS = {
     "b9_expire": (C.c_int64, [C.c_void_p, C.c_int64]),
     "b9_cancel": (C.c_int64, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]),
     "b9_set_retry_policy": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32]),
+    "b9_set_callback_policy": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_uint32]),
+    "b9_drain_fetch_callbacks": (C.c_int64, [C.c_void_p, C.POINTER(Results), C.POINTER(Callbacks)]),
     "b9_drain": (C.c_int64, [C.c_void_p, C.c_int, C.c_uint32, C.POINTER(Results)]),
     "b9_drain_launch": (C.c_int64, [C.c_void_p, C.c_int, C.c_uint32, C.c_int]),
     "b9_drain_fetch": (C.c_int64, [C.c_void_p, C.POINTER(Results)]),

@@ -42,6 +42,11 @@
 cudaError_t launch_wire_encode_full(const void* args, size_t args_size, const void* env, uint32_t grid, cudaStream_t s);
 // pickle_pass_kernel for B9_DRAIN_PICKLE_FULL, from function_drain.cu; args: the drain's DrainArgs
 cudaError_t launch_pickle_pass(const void* args, size_t args_size, int handler, int sm_count, cudaStream_t s);
+// callback_sign_kernel for b9_set_callback_policy, from callback_sign.cu; args: the drain's DrainArgs (tile_tasks as
+// launch_drain3 chose it), mid: the key's midstates (callback_midstates), keyed = 0: kinds only
+void callback_midstates(const uint8_t* key, uint32_t key_len, uint32_t mid[16]);
+cudaError_t launch_callback_sign(const void* args, size_t args_size, const uint32_t mid[16], int keyed, int64_t ts,
+                                 uint8_t* kind, uint8_t* digest, int sm_count, cudaStream_t s);
 // endpoint_drain_kernel for b9_endpoint_drain_launch, from endpoint_drain.cu; args: the drain's DrainArgs, with tile_tasks
 // = ENDPOINT_TILE_TASKS and n_tiles set for it
 cudaError_t launch_endpoint_drain(const void* args, size_t args_size, int handler, int sm_count, cudaStream_t s);
@@ -151,6 +156,10 @@ struct b9_ctx {
     uint4* d_retry_ids = nullptr;              // [max_drain_tasks] their ids
     uint8_t* d_retry_bytes = nullptr; uint64_t retry_bytes_cap = 0;   // their payload bytes (grow-only)
     void* d_retry_scan = nullptr; size_t retry_scan_cap = 0;          // cub scan scratch (grow-only)
+    // the callback policy (b9_set_callback_policy; set under out_mu) and the sign pass's outputs (allocated with the first policy)
+    bool cb_enabled = false, cb_keyed = false; uint32_t cb_mid[16] = {};
+    uint8_t* d_cb_kind = nullptr;              // [max_drain_tasks] b9_callback_kind per record
+    uint8_t* d_cb_digest = nullptr;            // [max_drain_tasks * 32] raw HMAC-SHA256 per record
     // ring bookkeeping (host)
     uint64_t head_task = 0, tail_task = 0;     // logical, monotonically increasing
     uint64_t write_pos = 0;                    // physical byte position of the next segment
@@ -184,6 +193,7 @@ struct b9_ctx {
     // results waiting on the device for b9_drain_fetch
     bool have_results = false, res_peek = false;
     bool res_retry = false;                    // the waiting results come from a drain launched under a retry policy
+    bool res_cb = false, res_cb_keyed = false; int64_t res_cb_ts = 0;   // ... with a callback pass: its keying and Unix seconds
     uint64_t res_gen = 0;                      // bumped whenever the waiting results change (launch, fetch commit)
     uint32_t res_n = 0, res_popped = 0; uint64_t res_bytes = 0, res_in_bytes = 0; float res_kernel_ms = 0.f;
     bool res_ids_in_ring = false; uint64_t res_head = 0;   // record j's id is the ring id of task res_head + j (DrainOut::ids_compacted == 0)
@@ -588,6 +598,29 @@ int b9_set_retry_policy(b9_ctx* c, uint32_t exc_mask, uint32_t max_retries) {
     return B9_OK;
 }
 
+int b9_set_callback_policy(b9_ctx* c, int enabled, const uint8_t* signing_key, uint32_t key_len) {
+    if (!c) return fail(B9_EINVAL, "b9_set_callback_policy: ctx is NULL");
+    if (enabled && key_len && !signing_key) return fail(B9_EINVAL, "b9_set_callback_policy: NULL signing_key with key_len %u", key_len);
+    OutLock out_lk(c);
+    if (enabled && !c->d_cb_kind) {
+        CU(cudaSetDevice(c->device));
+        const size_t md = c->max_drain_tasks;
+        cudaError_t e = cudaMalloc(&c->d_cb_kind, md);
+        if (e == cudaSuccess) e = cudaMalloc(&c->d_cb_digest, md * 32);
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            cudaFree(c->d_cb_kind); cudaFree(c->d_cb_digest);
+            c->d_cb_kind = nullptr; c->d_cb_digest = nullptr;
+            return fail(e == cudaErrorMemoryAllocation ? B9_ENOMEM : B9_EIO, "b9_set_callback_policy: %s", cudaGetErrorString(e));
+        }
+    }
+    c->cb_enabled = enabled != 0;
+    c->cb_keyed = c->cb_enabled && key_len != 0;
+    if (c->cb_keyed) callback_midstates(signing_key, key_len, c->cb_mid);
+    else memset(c->cb_mid, 0, sizeof c->cb_mid);
+    return B9_OK;
+}
+
 int b9_device_count(void) {
     int n = 0;
     if (cudaGetDeviceCount(&n) != cudaSuccess) { cudaGetLastError(); return 0; }
@@ -704,6 +737,7 @@ void b9_ctx_destroy(b9_ctx* c) {
     cudaFree(c->d_ctl); cudaFree(c->d_tile_state); cudaFree(c->d_count);
     cudaFree(c->d_cancel_keys); cudaFree(c->d_cancel_out);
     cudaFree(c->d_task_of); cudaFree(c->d_retry_rec); cudaFree(c->d_retry_ids); cudaFree(c->d_retry_bytes); cudaFree(c->d_retry_scan);
+    cudaFree(c->d_cb_kind); cudaFree(c->d_cb_digest);
     if (c->h_ctl) cudaFreeHost(c->h_ctl);
     if (c->h_rtab) cudaFreeHost(c->h_rtab);
     cudaFree(c->d_rtab); cudaFree(c->d_prefix); cudaFree(c->d_scan_sums);
@@ -1143,6 +1177,9 @@ static int64_t drain_launch_common(b9_ctx* c, int handler, uint32_t max_tasks, i
     c->running.store(0, std::memory_order_relaxed);
     c->res_n = 0; c->res_popped = 0; c->res_bytes = 0; c->res_in_bytes = 0; c->res_peek = (peek & B9_DRAIN_PEEK) != 0;
     c->res_gen++; c->res_retry = false;
+    // the callback pass signs with the host clock's Unix seconds, read once per launch (SignPayload's time.Now().Unix())
+    c->res_cb = !endpoint && c->cb_enabled; c->res_cb_keyed = c->res_cb && c->cb_keyed;
+    c->res_cb_ts = c->res_cb_keyed ? (int64_t)std::chrono::duration_cast<std::chrono::seconds>(std::chrono::system_clock::now().time_since_epoch()).count() : 0;
     cudaStream_t s = c->stream;
     // the window: a snapshot of the ring's head under the bookkeeping lock. Only drain-side calls (all under out_mu)
     // move the head or free segments, so the snapshot stays valid while the launch is prepared without c->mu.
@@ -1242,11 +1279,20 @@ static int64_t drain_launch_common(b9_ctx* c, int handler, uint32_t max_tasks, i
         a.tile_tasks = tt;
         le = launch_pickle_pass(&a, sizeof a, handler, c->sm_count, s);
         if (le != cudaSuccess) { c->last_op_drain = false; c->ctl_dirty = true; return fail(B9_EIO, "pickle pass launch failed: %s", cudaGetErrorString(le)); }
-        end_drain_span(c);
     }
+    // under a callback policy: every record's callback kind and signature (callback_sign.cu), behind the records' last
+    // writer (drain3_kernel or the pickle pass). Like the pickle pass it is never a programmatic dependent, the next drain
+    // kernel waits for it in full, and the timed span ends behind it. It reads this launch's control block and count
+    // prefixes, which nothing rewrites before the next launch.
+    if (c->res_cb) {
+        a.tile_tasks = tt;
+        le = launch_callback_sign(&a, sizeof a, c->cb_mid, c->res_cb_keyed ? 1 : 0, c->res_cb_ts, c->d_cb_kind, c->d_cb_digest, c->sm_count, s);
+        if (le != cudaSuccess) { c->last_op_drain = false; c->ctl_dirty = true; return fail(B9_EIO, "callback sign pass launch failed: %s", cudaGetErrorString(le)); }
+    }
+    if (pickle_pass || c->res_cb) end_drain_span(c);
     {
         std::lock_guard<std::mutex> lk(c->mu);
-        c->stats.kernel_launches += (a.count_mode ? 3 : 1) + (pickle_pass ? 1 : 0);   // (+ tile_count_kernel and tile_scan_kernel)
+        c->stats.kernel_launches += (a.count_mode ? 3 : 1) + (pickle_pass ? 1 : 0) + (c->res_cb ? 1 : 0);   // (+ tile_count_kernel and tile_scan_kernel)
         c->stats.last_drain_tiles = (n + 127) / 128;                       // (reported in units of 128 tasks)
         c->stats.drains++;
     }
@@ -1271,19 +1317,21 @@ int64_t b9_endpoint_drain_launch(b9_ctx* c, int handler, uint32_t max_tasks, int
     return drain_launch_common(c, handler, max_tasks, flags, true);
 }
 
-int64_t b9_drain_fetch(b9_ctx* c, b9_results* out) {
-    if (!c || !out) return fail(B9_EINVAL, "b9_drain_fetch: NULL argument");
+// b9_drain_fetch, and with cb (b9_drain_fetch_callbacks) the launch's callback kinds and digests in the same read-back
+static int64_t drain_fetch(b9_ctx* c, b9_results* out, b9_callbacks* cb) {
     std::unique_lock<std::mutex> in_lk(c->in_mu, std::defer_lock);
     std::unique_lock<std::mutex> out_lk(c->out_mu);
     end_drain_span(c);
     CU(cudaSetDevice(c->device));
     { int rc = finish_launch(c); if (rc) return rc; }
     if (!c->have_results) return fail(B9_EINVAL, "b9_drain_fetch: no drain results are waiting");
+    if (cb && !c->res_cb) return fail(B9_EINVAL, "b9_drain_fetch_callbacks: the waiting results come from a launch without a callback pass");
     out->n_results = c->res_n; out->n_popped = c->res_popped; out->n_bytes = c->res_bytes; out->need_bytes = c->res_bytes;
     out->task_duration = 0.f;
-    if (c->res_n > out->cap_tasks || c->res_bytes > out->cap_bytes)
-        return fail(B9_ENOSPC, "b9_drain_fetch: need %u records / %llu bytes, caller gave %u / %llu", c->res_n,
-                    (unsigned long long)c->res_bytes, out->cap_tasks, (unsigned long long)out->cap_bytes);
+    if (cb) cb->timestamp = c->res_cb_ts;
+    if (c->res_n > out->cap_tasks || c->res_bytes > out->cap_bytes || (cb && c->res_n > cb->cap_tasks))
+        return fail(B9_ENOSPC, "b9_drain_fetch: need %u records / %llu bytes, caller gave %u / %llu (callbacks: %u)", c->res_n,
+                    (unsigned long long)c->res_bytes, out->cap_tasks, (unsigned long long)out->cap_bytes, cb ? cb->cap_tasks : 0u);
     cudaStream_t s = c->stream;
     const size_t n = c->res_n;
     CU(cudaEventRecord(c->ev_c, s));
@@ -1302,6 +1350,12 @@ int64_t b9_drain_fetch(b9_ctx* c, b9_results* out) {
         if (c->res_bytes) {
             if (!out->payload) return fail(B9_EINVAL, "b9_drain_fetch: NULL payload buffer");
             CU(cudaMemcpyAsync(out->payload, c->d_out_payload, c->res_bytes, cudaMemcpyDeviceToHost, s));
+        }
+        if (cb) {
+            if (!cb->kind || !cb->digest) return fail(B9_EINVAL, "b9_drain_fetch_callbacks: NULL callback array");
+            CU(cudaMemcpyAsync(cb->kind, c->d_cb_kind, n, cudaMemcpyDeviceToHost, s));
+            if (c->res_cb_keyed) CU(cudaMemcpyAsync(cb->digest, c->d_cb_digest, n * 32, cudaMemcpyDeviceToHost, s));
+            else memset(cb->digest, 0, n * 32);                          // (without a key no digest is written)
         }
     }
     CU(cudaEventRecord(c->ev_d, s));
@@ -1332,13 +1386,23 @@ int64_t b9_drain_fetch(b9_ctx* c, b9_results* out) {
     } else {
         std::lock_guard<std::mutex> lk(c->mu);
         c->stats.last_drain_d2h_ms = ms;
-        c->stats.bytes_d2h += c->res_bytes + n * (16 + 1 + 1 + 8 + 4);
+        c->stats.bytes_d2h += c->res_bytes + n * (16 + 1 + 1 + 8 + 4) + (cb ? n * (1 + (c->res_cb_keyed ? 32 : 0)) : 0);
         if (!c->res_peek) commit_pop(c);
     }
     if (!c->res_peek && c->recount_cancelled) { int rc = recount_cancelled_locked_out(c); if (rc) return rc; }
     c->running.store(0, std::memory_order_relaxed);
     c->have_results = false; c->res_async = false; c->burst_open = false; c->res_gen++;
     return (int64_t)n;
+}
+
+int64_t b9_drain_fetch(b9_ctx* c, b9_results* out) {
+    if (!c || !out) return fail(B9_EINVAL, "b9_drain_fetch: NULL argument");
+    return drain_fetch(c, out, nullptr);
+}
+
+int64_t b9_drain_fetch_callbacks(b9_ctx* c, b9_results* out, b9_callbacks* cb) {
+    if (!c || !out || !cb) return fail(B9_EINVAL, "b9_drain_fetch_callbacks: NULL argument");
+    return drain_fetch(c, out, cb);
 }
 
 int64_t b9_drain(b9_ctx* c, int handler, uint32_t max_tasks, b9_results* out) {
@@ -1394,7 +1458,7 @@ static int64_t wire_encode(b9_ctx* c, const b9_wire_env* env, uint32_t max_tasks
         for (const Segment& sg : c->segs) CU(cudaStreamWaitEvent(s, sg.ready, 0));
     }
     c->res_n = 0; c->res_popped = 0; c->res_bytes = 0; c->res_in_bytes = 0; c->res_peek = true;
-    c->res_gen++; c->res_retry = false;
+    c->res_gen++; c->res_retry = false; c->res_cb = false;
     if (n == 0) { c->have_results = true; return 0; }
     WireEnv we; memset(&we, 0, sizeof we);
     {

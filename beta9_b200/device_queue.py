@@ -8,6 +8,7 @@ from __future__ import annotations
 
 import binascii
 import ctypes as C
+import uuid
 from dataclasses import dataclass
 from typing import Iterable, List, Optional, Tuple
 
@@ -46,6 +47,10 @@ class DrainResult:
     payload: np.ndarray      # uint8 [n_bytes]  byte order = tile completion order (16-byte padded ranges), use offsets
     n_popped: int
     task_duration: float = 0.0   # seconds charged to every task of the drain (TaskQueueCompleteRequest.task_duration)
+    # with callbacks=True (b9_drain_fetch_callbacks): the runner's callback per record
+    cb_kind: Optional[np.ndarray] = None     # uint8 [n]     CB_NONE / CB_POST / CB_UNSENDABLE / CB_HOST
+    cb_digest: Optional[np.ndarray] = None   # uint8 [n,32]  raw HMAC-SHA256 of a CB_POST record under a key, else zero
+    cb_timestamp: int = 0                    # the Unix seconds every digest signs (0: no key)
 
     @property
     def n(self) -> int:
@@ -67,6 +72,18 @@ class DrainResult:
         rec = np.repeat(np.arange(self.n, dtype=np.int64), ln)
         src = self.offsets.astype(np.int64)[rec] + (idx - (ends - ln)[rec])
         return self.payload[src]
+
+    def callback_body(self, i: int) -> bytes:
+        """The bytes the runner signs and posts for record i: {"data": R}, or {"data": {}} without result bytes."""
+        r = self.result(i)
+        return b'{"data": ' + (r if r is not None else b"{}") + b"}"
+
+    def callback_headers(self, i: int, status: Optional[str] = None) -> dict:
+        """send_callback's headers for record i (status: the runner's TaskStatus, by default the record's)."""
+        sig = self.cb_digest[i].tobytes().hex() if self.cb_timestamp else ""
+        return {"X-Task-ID": str(uuid.UUID(bytes=self.task_ids[i].tobytes())),
+                "X-Task-Status": status or STATUS_NAMES[int(self.status[i])],
+                "X-Task-Signature": sig, "X-Task-Timestamp": str(self.cb_timestamp)}
 
     def records(self) -> List[Tuple[bytes, str, Optional[bytes]]]:
         return [(self.task_ids[i].tobytes(), STATUS_NAMES[int(self.status[i])], self.result(i)) for i in range(self.n)]
@@ -187,6 +204,16 @@ class DeviceQueue:
         marked = self._check(self._lib.b9_cancel(self._ctx, ids.ctypes.data if n else None, n, outcome.ctypes.data))
         return marked, outcome[:n]
 
+    def set_callback_policy(self, signing_key: Optional[bytes]) -> None:
+        """b9_set_callback_policy: the stub has a callback URL and its workspace signs with `signing_key` (b"": the gateway
+        without a key; the runner then posts unsigned). None turns the callback pass off. Drains launched after it run
+        the pass; fetch them with callbacks=True."""
+        if signing_key is None:
+            self._check(self._lib.b9_set_callback_policy(self._ctx, 0, None, 0))
+        else:
+            key = bytes(signing_key)
+            self._check(self._lib.b9_set_callback_policy(self._ctx, 1, key if key else None, len(key)))
+
     def set_retry_policy(self, retry_for: Optional[Iterable[type]], max_retries: int) -> None:
         """b9_set_retry_policy: the stub's `retry_for` classes and TaskPolicy.MaxRetries. A task whose handler raised one of
         them comes back RETRY (and is pushed again, retries + 1, when its drain is fetched) or, once its retries reached
@@ -196,11 +223,12 @@ class DeviceQueue:
 
     # ---- consumer side
     def drain(self, handler: str, max_tasks: int = 1 << 22, cap_bytes: Optional[int] = None, full_pickle: bool = False,
-              endpoint: bool = False) -> DrainResult:
+              endpoint: bool = False, callbacks: bool = False) -> DrainResult:
         """full_pickle=True (B9_DRAIN_PICKLE_FULL): pickle-framed tasks of every handler over plain values (include/b9gpu.h).
-        endpoint=True (b9_endpoint_drain_launch): B9_TF_HTTP_BODY tasks answered with the endpoint runner's response bodies."""
+        endpoint=True (b9_endpoint_drain_launch): B9_TF_HTTP_BODY tasks answered with the endpoint runner's response bodies.
+        callbacks=True (b9_drain_fetch_callbacks, under set_callback_policy): the result carries each record's callback."""
         n = self._launch(HANDLERS[handler], max_tasks, L.DRAIN_PICKLE_FULL if full_pickle else 0, endpoint)
-        return self._fetch(n, cap_bytes)
+        return self._fetch(n, cap_bytes, callbacks)
 
     def drain_launch(self, handler: str, max_tasks: int = 1 << 22, peek: bool = False, wait: bool = True, full_pickle: bool = False,
                      endpoint: bool = False) -> int:
@@ -215,12 +243,12 @@ class DeviceQueue:
             raise ValueError("endpoint=True answers HTTP bodies only: it does not combine with full_pickle=True")
         return self._check(self._lib.b9_endpoint_drain_launch(self._ctx, h, max_tasks, flags))
 
-    def fetch(self, cap_bytes: Optional[int] = None) -> DrainResult:
+    def fetch(self, cap_bytes: Optional[int] = None, callbacks: bool = False, cap_tasks: Optional[int] = None) -> DrainResult:
         self.sync()                                  # completes a wait=False launch: its byte count sizes the buffers below
         st = self.stats()
-        return self._fetch(None, cap_bytes if cap_bytes is not None else int(st.last_drain_out_bytes))
+        return self._fetch(cap_tasks, cap_bytes if cap_bytes is not None else int(st.last_drain_out_bytes), callbacks)
 
-    def _fetch(self, n: Optional[int], cap_bytes: Optional[int]) -> DrainResult:
+    def _fetch(self, n: Optional[int], cap_bytes: Optional[int], callbacks: bool = False) -> DrainResult:
         st = self.stats()
         if cap_bytes is None:
             cap_bytes = int(st.last_drain_out_bytes)
@@ -234,8 +262,15 @@ class DeviceQueue:
         pl = np.empty(max(cap_bytes, 1), np.uint8)
         r = L.Results(ids.ctypes.data, status.ctypes.data, has.ctypes.data, off.ctypes.data, ln.ctypes.data, pl.ctypes.data,
                       max(n, 1), max(cap_bytes, 1), 0, 0, 0, 0, 0.0, 0)
-        got = self._check(self._lib.b9_drain_fetch(self._ctx, C.byref(r)))
-        return DrainResult(ids[:got], status[:got], has[:got], off[:got], ln[:got], pl[:int(r.n_bytes)], int(r.n_popped), float(r.task_duration))
+        if not callbacks:
+            got = self._check(self._lib.b9_drain_fetch(self._ctx, C.byref(r)))
+            return DrainResult(ids[:got], status[:got], has[:got], off[:got], ln[:got], pl[:int(r.n_bytes)], int(r.n_popped), float(r.task_duration))
+        kind = np.empty(max(n, 1), np.uint8)
+        digest = np.empty((max(n, 1), 32), np.uint8)
+        cb = L.Callbacks(kind.ctypes.data, digest.ctypes.data, max(n, 1), 0)
+        got = self._check(self._lib.b9_drain_fetch_callbacks(self._ctx, C.byref(r), C.byref(cb)))
+        return DrainResult(ids[:got], status[:got], has[:got], off[:got], ln[:got], pl[:int(r.n_bytes)], int(r.n_popped), float(r.task_duration),
+                           kind[:got], digest[:got], int(cb.timestamp))
 
     def drain_object(self, handler: str, max_tasks: int = 1 << 22, endpoint: bool = False) -> np.ndarray:
         """One drain whose records land as ONE result-sink object (b9_drain_fetch_object): header + index + blob."""

@@ -12,6 +12,9 @@ CPU fallback: tasks the device handler does not implement come back with status 
 """
 from __future__ import annotations
 
+import base64
+import hashlib
+import hmac
 import json
 import os
 import uuid
@@ -35,6 +38,9 @@ class Task:
     status: str = "PENDING"
     result: Any = None
     result_bytes: Optional[bytes] = None
+    # with a stub callback_url: what the runner hands requests.post after this task, (url, body bytes, headers); None
+    # where it posts nothing (RETRY, a body requests refuses) or where the device did not settle the task (UNSUPPORTED)
+    callback: Optional[tuple] = None
 
     def raw_id(self) -> bytes:
         return uuid.UUID(self.id).bytes
@@ -44,12 +50,15 @@ class TaskQueue:
     """Decorator. Resource arguments are accepted and kept for API compatibility; only the ones
     this path reads have an effect (`max_pending_tasks`, `retries`, `retry_for`, `gpu_handler`, `device`). A task whose
     handler raises a class in `retry_for` (an exact match, as the runner's retry_on_errors) comes back "RETRY" and is
-    queued again, up to `retries` times; after that it comes back "RETRY_LIMIT" (the gateway cancels it)."""
+    queued again, up to `retries` times; after that it comes back "RETRY_LIMIT" (the gateway cancels it). With
+    `callback_url`, every drained task carries the callback the runner would post (Task.callback), signed with the
+    workspace's `signing_key` (None or b"": unsigned, as a gateway without a key); nothing is posted here."""
 
     def __init__(self, cpu: Union[int, float, str] = 1.0, memory: Union[int, str] = 128, gpu: Any = "", image: Any = None,
                  timeout: int = 3600, retries: int = 3, workers: int = 1, keep_warm_seconds: int = 10,
                  max_pending_tasks: int = DEFAULT_MAX_PENDING_TASKS, name: Optional[str] = None,
-                 retry_for: Optional[List[type]] = None, gpu_handler: Optional[str] = None, device: int = 0, queue: Optional[DeviceQueue] = None, **kwargs: Any):
+                 retry_for: Optional[List[type]] = None, gpu_handler: Optional[str] = None, device: int = 0, queue: Optional[DeviceQueue] = None,
+                 callback_url: Optional[str] = None, signing_key: Optional[bytes] = None, **kwargs: Any):
         self.cpu = int(float(cpu) * 1000) if not isinstance(cpu, str) else cpu     # base/runner.py parse_cpu: cores -> millicores
         self.memory = memory
         self.gpu = gpu
@@ -57,6 +66,8 @@ class TaskQueue:
         self.timeout = timeout
         self.retries = retries
         self.retry_for = list(retry_for or [])
+        self.callback_url = callback_url
+        self.signing_key = bytes(signing_key or b"")
         self.workers = workers
         self.keep_warm_seconds = keep_warm_seconds
         self.max_pending_tasks = max_pending_tasks
@@ -74,6 +85,8 @@ class TaskQueue:
             self._queue = DeviceQueue(device=self.device)     # raises without a GPU: no CPU path
         if not self._policy_set:
             self._queue.set_retry_policy(self.retry_for, self.retries)
+            if self.callback_url:
+                self._queue.set_callback_policy(self.signing_key)
             self._policy_set = True
         return self._queue
 
@@ -90,6 +103,7 @@ class _CallableWrapper:
         self.func = func
         self.parent = parent
         self._held: List[Task] = []       # drained on behalf of a map(): handed out by the next process_tasks()
+        self._cb_override: Dict[str, Any] = {}   # task id -> its "callback_url" kwarg (the device leaves those to the host)
 
     def __call__(self, *args: Any, **kwargs: Any) -> Any:
         # sdk taskqueue.py:218-224: callable only inside a container
@@ -126,6 +140,8 @@ class _CallableWrapper:
             return []
         payloads = [self._payload(a, k) for a, k in norm]
         ids = [uuid.uuid4() for _ in norm]
+        if self.parent.callback_url:
+            self._cb_override.update((str(i), k["callback_url"]) for i, (_, k) in zip(ids, norm) if "callback_url" in k)
         offsets = np.zeros(len(norm) + 1, np.uint64)
         np.cumsum([len(p) for p in payloads], out=offsets[1:])
         blob = np.frombuffer(b"".join(payloads), np.uint8)
@@ -188,13 +204,36 @@ class _CallableWrapper:
         return out
 
     def _drain(self, max_tasks: int) -> List[Task]:
-        res = self.parent.queue.drain(self.parent.gpu_handler, max_tasks=max_tasks)
+        cb = bool(self.parent.callback_url)
+        q = self.parent.queue
+        res = q.drain(self.parent.gpu_handler, max_tasks=max_tasks, callbacks=True) if cb else q.drain(self.parent.gpu_handler, max_tasks=max_tasks)
         out = []
         for i in range(res.n):
             rb = res.result(i)
-            out.append(Task(id=str(uuid.UUID(bytes=res.task_ids[i].tobytes())), status=STATUS_NAMES[int(res.status[i])],
-                            result=json.loads(rb) if rb is not None else None, result_bytes=rb))
+            t = Task(id=str(uuid.UUID(bytes=res.task_ids[i].tobytes())), status=STATUS_NAMES[int(res.status[i])],
+                     result=json.loads(rb) if rb is not None else None, result_bytes=rb)
+            if cb:
+                t.callback = self._callback(res, i, t)
+            out.append(t)
         return out
+
+    def _callback(self, res, i: int, t: Task) -> Optional[tuple]:
+        """send_callback's request for record i (runner/common.py:430-481): the device's signature for B9_CB_POST; the one
+        kind the host settles here is an ERROR whose kwargs carried "callback_url" (the runner's override), signed on the
+        CPU as SignPayload does (pkg/auth/sign.go:17-35)."""
+        kind = int(res.cb_kind[i])
+        override = self._cb_override.pop(t.id, None)
+        if kind == L.CB_POST:
+            return self.parent.callback_url, res.callback_body(i), res.callback_headers(i)
+        if kind == L.CB_HOST and t.status == "ERROR":
+            url = override or self.parent.callback_url
+            body = res.callback_body(i)
+            key, ts = self.parent.signing_key, res.cb_timestamp
+            sig = hmac.new(key, base64.b64encode(body) + b":%d" % ts, hashlib.sha256).hexdigest() if key else ""
+            headers = res.callback_headers(i)
+            headers["X-Task-Signature"] = sig
+            return url, body, headers
+        return None
 
     def map(self, inputs: Sequence[Any]) -> Iterator[Any]:
         """Fan out: one task per input, one push, then drains until every one of ITS tasks has come back; yields each

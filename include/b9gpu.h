@@ -319,6 +319,42 @@ int64_t  b9_cancel(b9_ctx *ctx, const uint8_t *task_ids, uint32_t n, uint8_t *ou
  * Added without an ABI version change: probe for it with dlsym. */
 int      b9_set_retry_policy(b9_ctx *ctx, uint32_t exc_mask, uint32_t max_retries);
 
+/* ---- task callbacks: the runner's send_callback and the gateway's SignPayload, per drained record ----------------------
+ * A stub declared with callback_url= gets a request after every task it completes (sdk/src/beta9/runner/taskqueue.py:
+ * 391-397, runner/common.py:430-481): POST {"data": result or {}} with X-Task-ID, X-Task-Status, X-Task-Signature and
+ * X-Task-Timestamp, the signature being hex(HMAC-SHA256(workspace signing key, base64(body) + ":" + Unix seconds))
+ * (pkg/auth/sign.go:17-35). Under a policy, every b9_drain_launch runs one more pass over its records that settles which
+ * callback the runner sends and signs it. Per record of the task-queue drain:
+ *   B9_CB_POST        COMPLETE with result bytes R: body = {"data": R}; COMPLETE without (a falsy result) and ERROR:
+ *                     body = {"data": {}}. Signed bytes = posted bytes = the body.
+ *   B9_CB_UNSENDABLE  COMPLETE whose R is NaN / Infinity / -Infinity (json_sum's overflowing totals): the runner signs it,
+ *                     then requests refuses the body (allow_nan=False) and nothing is posted.
+ *   B9_CB_NONE        RETRY, RETRY_LIMIT (the runner continues before the callback) and REJECTED (no task exists).
+ *   B9_CB_HOST        not settled on the device: UNSUPPORTED, every B9_TF_PICKLE task, and an ERROR whose kwargs hold a
+ *                     "callback_url" key (the runner posts to that value, or to the stub's URL when it is falsy).
+ * The body is always the bytes {"data":  (9 bytes with the space), then R or {}, then }: the host builds it from the
+ * record. Headers: X-Task-ID = the record id as canonical UUID text, X-Task-Status = COMPLETE / ERROR, X-Task-Signature =
+ * the lower-case hex of the digest, X-Task-Timestamp = b9_callbacks.timestamp. */
+enum b9_callback_kind { B9_CB_NONE = 0, B9_CB_POST = 1, B9_CB_UNSENDABLE = 2, B9_CB_HOST = 3 };
+/* The stub has a callback URL (enabled = 1), signed with the workspace's key; key_len 0 is the gateway without a key
+ * (SignPayload answers Ok: false): the runner still posts, with X-Task-Signature "" and X-Task-Timestamp 0, so the pass
+ * writes no digests and reports timestamp 0. A key longer than 64 bytes is hashed first, as Go's hmac.New does. Applies to
+ * the b9_drain_launch calls made after it (a drain-side call); enabled = 0, the default, launches exactly what a drain
+ * without a policy launches. Not affected: b9_endpoint_drain_launch. Returns 0, or B9_EINVAL (NULL ctx, NULL key with
+ * key_len > 0), B9_ENOMEM. Added without an ABI version change: probe for it with dlsym. */
+int      b9_set_callback_policy(b9_ctx *ctx, int enabled, const uint8_t *signing_key, uint32_t key_len);
+typedef struct b9_callbacks {
+    uint8_t *kind;        /* [cap_tasks]    enum b9_callback_kind, record order                          */
+    uint8_t *digest;      /* [cap_tasks*32] raw HMAC-SHA256 for B9_CB_POST under a key, else zero        */
+    uint32_t cap_tasks;
+    int64_t  timestamp;   /* filled: the Unix seconds every digest of this drain signs (0: no key); the host
+                             clock, read once by each b9_drain_launch that runs under a policy             */
+} b9_callbacks;
+/* b9_drain_fetch plus the launch's callbacks in the same read-back: the same records, commit and B9_ENOSPC (nothing is
+ * consumed when either the results or `cb` are too small). B9_EINVAL when the fetched launch ran no callback pass (no
+ * policy, b9_endpoint_drain_launch, the wire encoders). After a burst of B9_DRAIN_ASYNC launches, the last one's. */
+int64_t  b9_drain_fetch_callbacks(b9_ctx *ctx, b9_results *out, b9_callbacks *cb);
+
 /* ---- consumer side ---------------------------------------------------------------------------
  * b9_drain replaces, for up to max_tasks pending tasks in FIFO order, the whole
  *   TaskQueuePop (taskqueue.go:228-310, client.go:43-96)
