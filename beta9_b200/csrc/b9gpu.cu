@@ -422,7 +422,10 @@ void commit_pop(b9_ctx* c) {
 // The re-push's device half, for retried task k = the window task (task_of) of record rec[k]. retry_len_kernel, one thread
 // per task: rel[k + 1] = its length (a scan then makes rel the exclusive byte prefix). retry_gather_kernel, one warp per
 // task: its bytes are copied out of the claimed window into the scratch `bytes` at rel[k], with the slot words
-// ingest_kernel writes for a push: retries + 1, the commit's timestamp, the same expiry, flags and id.
+// ingest_kernel writes for a push: retries + 1, the commit's timestamp, the same expiry, flags and id. The flags are the
+// ones the task was pushed with: a task pushed cancelled leaves no record, so a CANCELLED bit here was set by a
+// b9_expire sweep of the claimed window, and it is cleared. The reference's monitor expires only unclaimed tasks
+// (dispatch.go:173-230) and RetryTask re-queues the task as it was; the kept expiry cancels it at the next b9_expire.
 __global__ void retry_len_kernel(const uint32_t* __restrict__ rec, uint32_t n, const uint32_t* __restrict__ task_of, const uint64_t* __restrict__ hdr,
                                  uint64_t head, uint32_t slot_mask, uint64_t* __restrict__ rel) {
     const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
@@ -440,7 +443,7 @@ __global__ void retry_gather_kernel(const uint32_t* __restrict__ rec, uint32_t n
     const uint64_t h = hdr[slot];
     warp_copy(bytes + rel[k], payload + off[slot], hdr_len(h), (int)lane);
     if (lane == 0) {
-        o_ts[k] = now_unix; o_exp[k] = exp[slot]; o_retries[k] = (uint8_t)(hdr_retries(h) + 1u); o_flags[k] = (uint8_t)hdr_flags(h); o_ids[k] = ids[slot];
+        o_ts[k] = now_unix; o_exp[k] = exp[slot]; o_retries[k] = (uint8_t)(hdr_retries(h) + 1u); o_flags[k] = (uint8_t)(hdr_flags(h) & ~B9_TF_CANCELLED); o_ids[k] = ids[slot];
     }
 }
 
@@ -449,8 +452,8 @@ __global__ void retry_gather_kernel(const uint32_t* __restrict__ rec, uint32_t n
 // fetched. Everything runs on the ingest stream, behind earlier pushes and ahead of later ones: the tasks are gathered out
 // of the claimed window into scratch, then the space is placed in the same critical section that commits the pop (a
 // producer cannot take the released space in between), then the bytes and slot words go to the new segment. When the
-// ring has no room for it, nothing is committed: B9_ENOSPC.
-int commit_with_repush(b9_ctx* c, const std::vector<uint32_t>& retry_rec, float d2h_ms) {
+// ring has no room for it, nothing is committed: B9_ENOSPC. d2h_bytes: what the fetch read back, for the stats.
+int commit_with_repush(b9_ctx* c, const std::vector<uint32_t>& retry_rec, float d2h_ms, uint64_t d2h_bytes) {
     const uint32_t k = (uint32_t)retry_rec.size();
     cudaStream_t s = c->stream_in;
     const uint64_t head = c->res_head;
@@ -536,7 +539,7 @@ int commit_with_repush(b9_ctx* c, const std::vector<uint32_t>& retry_rec, float 
     for (int q = 0; q < n_plan; ++q) if (!ready[q]) CU(cudaEventCreateWithFlags(&ready[q], cudaEventDisableTiming));
     std::lock_guard<std::mutex> lk(c->mu);
     c->stats.last_drain_d2h_ms = d2h_ms;
-    c->stats.bytes_d2h += c->res_bytes + (uint64_t)c->res_n * (16 + 1 + 1 + 8 + 4);
+    c->stats.bytes_d2h += d2h_bytes;
     commit_pop(c);
     if (partial)
         for (Segment& sg : c->segs)
@@ -1368,6 +1371,8 @@ static int64_t drain_fetch(b9_ctx* c, b9_results* out, b9_callbacks* cb) {
     // TaskQueueCompleteRequest.task_duration (taskqueue.proto:50): the runner reports the seconds it spent on a task; a
     // drain spends kernel + read-back time on res_popped tasks at once, so every task of the batch is charged its share
     if (c->res_popped) out->task_duration = (c->res_kernel_ms + ms) * 1e-3f / (float)c->res_popped;
+    // the records, and with cb the kinds and (under a key) the digests
+    const uint64_t d2h_bytes = c->res_bytes + n * (16 + 1 + 1 + 8 + 4) + (cb ? n * (1 + (c->res_cb_keyed ? 32 : 0)) : 0);
     if (!retry_rec.empty()) {
         // the re-push is a push: it takes the producers' lock, so that concurrent pushes land wholly before or after it. The
         // lock order is in_mu before out_mu: when a producer holds in_mu, out_mu is let go while the fetch waits for it, and
@@ -1381,12 +1386,12 @@ static int64_t drain_fetch(b9_ctx* c, b9_results* out, b9_callbacks* cb) {
             if (c->res_gen != gen || !c->have_results)
                 return fail(B9_EINVAL, "b9_drain_fetch: another drain-side call replaced or committed these results meanwhile");
         }
-        const int rc = commit_with_repush(c, retry_rec, ms);
+        const int rc = commit_with_repush(c, retry_rec, ms, d2h_bytes);
         if (rc) return rc;
     } else {
         std::lock_guard<std::mutex> lk(c->mu);
         c->stats.last_drain_d2h_ms = ms;
-        c->stats.bytes_d2h += c->res_bytes + n * (16 + 1 + 1 + 8 + 4) + (cb ? n * (1 + (c->res_cb_keyed ? 32 : 0)) : 0);
+        c->stats.bytes_d2h += d2h_bytes;
         if (!c->res_peek) commit_pop(c);
     }
     if (!c->res_peek && c->recount_cancelled) { int rc = recount_cancelled_locked_out(c); if (rc) return rc; }
