@@ -19,6 +19,7 @@
 #include <atomic>
 #include <condition_variable>
 #include <functional>
+#include <memory>
 #include <mutex>
 #include <thread>
 #include <new>
@@ -71,14 +72,56 @@ int fail(int code, const char* fmt, ...) {
 uint64_t pow2_ceil(uint64_t v) { uint64_t p = 1; while (p < v) p <<= 1; return p; }
 void nccl_comm_destroy(void* comm);   // defined with the NCCL loader below
 
+// Owning holders of the context's CUDA resources: what they hold is released when they are destroyed (b9_ctx_destroy sets
+// the device first) or reset. They convert to the raw handle, so the code that uses them reads as with a plain one.
+template <class H, cudaError_t (*Release)(H)> struct Owned {
+    H v{};
+    Owned() = default;
+    Owned(const Owned&) = delete;
+    Owned& operator=(const Owned&) = delete;
+    ~Owned() { reset(); }
+    void reset() { if (v) Release(v); v = H{}; }
+    operator H() const { return v; }
+    H operator->() const { return v; }
+};
+template <class T> cudaError_t free_device(T* p) { return cudaFree(p); }
+template <class T> cudaError_t free_pinned(T* p) { return cudaFreeHost(p); }
+template <class T> using DevPtr = Owned<T*, free_device<T>>;       // cudaMalloc
+template <class T> using PinnedPtr = Owned<T*, free_pinned<T>>;    // cudaHostAlloc
+using Event = Owned<cudaEvent_t, cudaEventDestroy>;
+using Stream = Owned<cudaStream_t, cudaStreamDestroy>;
+
+// Device (or page-locked) memory allocated on first use and grow-only: grow(need) keeps the buffer while it holds `need`
+// bytes, else replaces it with need + headroom bytes, or with nothing when that fails (the sticky error is cleared).
+// ensure() is grow() with a failure reported through fail(): B9_ENOMEM when the memory is short, else B9_EIO, with `what`
+// as the message.
+template <class T, bool Pinned = false> struct GrowBuf {
+    Owned<T*, Pinned ? free_pinned<T> : free_device<T>> p; uint64_t cap = 0;
+    operator T*() const { return p; }
+    cudaError_t grow(uint64_t need, uint64_t headroom = 0) {
+        if (need <= cap) return cudaSuccess;
+        p.reset(); cap = 0;
+        const cudaError_t e = Pinned ? cudaHostAlloc(&p.v, need + headroom, cudaHostAllocDefault) : cudaMalloc(&p.v, need + headroom);
+        if (e != cudaSuccess) { p.v = nullptr; cudaGetLastError(); return e; }
+        cap = need + headroom;
+        return cudaSuccess;
+    }
+    int ensure(uint64_t need, const char* what, uint64_t headroom = 0) {
+        const cudaError_t e = grow(need, headroom);
+        if (e == cudaSuccess) return B9_OK;
+        return fail(e == cudaErrorMemoryAllocation ? B9_ENOMEM : B9_EIO, "%s: %llu bytes: %s", what, (unsigned long long)(need + headroom),
+                    cudaGetErrorString(e));
+    }
+};
+
 struct Segment {             // one push = one contiguous byte range of the payload ring
     uint64_t first_task;     // logical index of its first task
     uint32_t n;
     uint64_t phys_start, bytes;
     cudaEvent_t ready;           // recorded on the ingest stream once the batch is fully on the device
-    uint32_t max_len = 0;        // longest task of the batch (0 = not known: tasks that arrived in a rebalance)
+    uint32_t max_len;            // longest task of the batch (0 = not known: tasks that arrived in a rebalance)
+    uint32_t n_pickle;           // tasks of the batch carrying B9_TF_PICKLE (all of them when not known: a rebalance)
     bool drain_waited = false;   // a drain launch has made the drain stream wait for `ready` (stream order covers later launches)
-    uint32_t n_pickle = 0;       // tasks of the batch carrying B9_TF_PICKLE (all of them when not known: a rebalance)
 };
 
 constexpr uint64_t RING_SLACK = 256;   // readable bytes past the ring end (vector loads may over-read)
@@ -113,9 +156,19 @@ struct PackPool {
 // page-locked staging of one packed batch (b9_batch_push_v): two of them alternate, so that batch k+1 is gathered
 // while batch k is still on the wire
 struct PackArena {
-    uint8_t* payload = nullptr; uint64_t cap_bytes = 0;
-    uint64_t* offsets = nullptr; uint8_t* ids = nullptr; uint32_t cap_tasks = 0;
-    cudaEvent_t free_ev = nullptr; bool in_flight = false;
+    GrowBuf<uint8_t, true> payload, ids; GrowBuf<uint64_t, true> offsets;
+    Event free_ev; bool in_flight = false;
+};
+
+// results waiting on the device for b9_drain_fetch; dropping them is `res = WaitingResults{}`
+struct WaitingResults {
+    bool have = false, peek = false;
+    bool retry = false;                        // they come from a drain launched under a retry policy
+    bool cb = false, cb_keyed = false; int64_t cb_ts = 0;   // ... with a callback pass: its keying and Unix seconds
+    uint32_t n = 0, popped = 0; uint64_t bytes = 0, in_bytes = 0; float kernel_ms = 0.f;
+    bool ids_in_ring = false; uint64_t head = 0;   // record j's id is the ring id of task head + j (DrainOut::ids_compacted == 0)
+    bool async = false;                        // the last launch returned before its kernels finished: finalize on fetch / sync
+    uint32_t async_n = 0; uint64_t async_in_bytes = 0;
 };
 
 }  // namespace
@@ -124,42 +177,42 @@ struct b9_ctx {
     int device = 0;
     int sm_count = 0;
     uint32_t stage_bytes_override = 0; // B9_STAGE_BYTES: force the v2 stage-buffer size
-    cudaStream_t stream = nullptr;             // drain kernels + D2H
-    cudaStream_t stream_in = nullptr;          // H2D + ingest kernel (so that pushes overlap drains: PCIe is full duplex)
-    std::vector<cudaEvent_t> event_pool;
-    cudaEvent_t ev_a = nullptr, ev_b = nullptr, ev_c = nullptr, ev_d = nullptr;   // drain stream (under out_mu)
-    cudaEvent_t ev_pa = nullptr, ev_pb = nullptr;                                    // ingest stream (under in_mu)
+    Stream stream;                             // drain kernels + D2H
+    Stream stream_in;                          // H2D + ingest kernel (so that pushes overlap drains: PCIe is full duplex)
+    std::vector<cudaEvent_t> event_pool;       // idle segment events (take_event / put_event)
+    Event ev_a, ev_b, ev_c, ev_d;              // drain stream (under out_mu)
+    Event ev_pa, ev_pb;                        // ingest stream (under in_mu)
     // Three locks, always taken in this order: in_mu (push submission: H2D + ingest kernel are enqueued in FIFO order),
     // out_mu (drain-side submission and the waiting-results state: launch, fetch, expire, cancel, wire records, rebalance), mu
     // (ring bookkeeping + stats; held for pointer arithmetic only, never across a CUDA synchronisation). Producers
     // therefore never wait for a drain's kernels or its D2H copy, and the drainer never waits for a push's DMA
     // (Dispatcher.Register's goroutine-safety contract, pkg/task/dispatch.go:71-73).
     std::mutex in_mu, out_mu, mu;
-    std::mutex pack_mu; PackPool* pack_pool = nullptr; PackArena pack[2]; int pack_next = 0;
+    std::mutex pack_mu; std::unique_ptr<PackPool> pack_pool; PackArena pack[2]; int pack_next = 0;
     // micro-batching of single-task submissions (b9_submit / b9_flush): two page-locked arenas, lock-free appends
-    std::mutex sb_mu; SubmitBuffer* sb = nullptr; cudaEvent_t sb_free[2] = {nullptr, nullptr}; bool sb_in_flight[2] = {false, false};
+    std::mutex sb_mu; std::unique_ptr<SubmitBuffer> sb; Event sb_free[2]; bool sb_in_flight[2] = {false, false};
     int sb_unpushed = -1; uint32_t sb_unpushed_n = 0;   // an arena whose push was refused (ring full): pushed again by the next flush
     std::atomic<uint64_t> running{0};           // tasks a drain has claimed (launched, not peeking) and not yet committed by a fetch
 
     // ---- pending ring (device)
     uint64_t ring_bytes = 0; uint32_t ring_tasks = 0, slot_mask = 0, max_task_bytes = 0;
-    uint8_t*  d_payload = nullptr;
-    uint64_t* d_off = nullptr; uint64_t* d_hdr = nullptr; uint4* d_ids = nullptr;
-    int64_t*  d_ts = nullptr;  int64_t* d_exp = nullptr;
+    DevPtr<uint8_t>  d_payload;
+    DevPtr<uint64_t> d_off; DevPtr<uint64_t> d_hdr; DevPtr<uint4> d_ids;
+    DevPtr<int64_t>  d_ts;  DevPtr<int64_t> d_exp;
     // push staging (device): raw offsets + optional metadata of the batch being ingested
-    uint64_t* d_in_off = nullptr; int64_t* d_in_ts = nullptr; int64_t* d_in_exp = nullptr;
-    uint8_t*  d_in_retries = nullptr; uint8_t* d_in_flags = nullptr;
+    DevPtr<uint64_t> d_in_off; DevPtr<int64_t> d_in_ts; DevPtr<int64_t> d_in_exp;
+    DevPtr<uint8_t>  d_in_retries; DevPtr<uint8_t> d_in_flags;
     // the retry policy (b9_set_retry_policy; set under out_mu) and the re-push's device buffers (allocated with the first policy)
     uint32_t retry_mask = 0, max_retries = 0;
-    uint32_t* d_task_of = nullptr;             // [max_drain_tasks] DrainArgs::task_of
-    uint32_t* d_retry_rec = nullptr;           // [max_drain_tasks] the RETRY records of a fetch, in record order
-    uint4* d_retry_ids = nullptr;              // [max_drain_tasks] their ids
-    uint8_t* d_retry_bytes = nullptr; uint64_t retry_bytes_cap = 0;   // their payload bytes (grow-only)
-    void* d_retry_scan = nullptr; size_t retry_scan_cap = 0;          // cub scan scratch (grow-only)
+    GrowBuf<uint32_t> d_task_of;               // [max_drain_tasks] DrainArgs::task_of
+    GrowBuf<uint32_t> d_retry_rec;             // [max_drain_tasks] the RETRY records of a fetch, in record order
+    GrowBuf<uint4> d_retry_ids;                // [max_drain_tasks] their ids
+    GrowBuf<uint8_t> d_retry_bytes;            // their payload bytes
+    GrowBuf<void> d_retry_scan;                // cub scan scratch
     // the callback policy (b9_set_callback_policy; set under out_mu) and the sign pass's outputs (allocated with the first policy)
     bool cb_enabled = false, cb_keyed = false; uint32_t cb_mid[16] = {};
-    uint8_t* d_cb_kind = nullptr;              // [max_drain_tasks] b9_callback_kind per record
-    uint8_t* d_cb_digest = nullptr;            // [max_drain_tasks * 32] raw HMAC-SHA256 per record
+    GrowBuf<uint8_t> d_cb_kind;                // [max_drain_tasks] b9_callback_kind per record
+    GrowBuf<uint8_t> d_cb_digest;              // [max_drain_tasks * 32] raw HMAC-SHA256 per record
     // ring bookkeeping (host)
     uint64_t head_task = 0, tail_task = 0;     // logical, monotonically increasing
     uint64_t write_pos = 0;                    // physical byte position of the next segment
@@ -168,51 +221,100 @@ struct b9_ctx {
 
     // ---- drain staging (device)
     uint32_t max_drain_tasks = 0; uint64_t max_result_bytes = 0;
-    uint8_t* d_out_payload = nullptr; uint64_t* d_out_off = nullptr; uint4* d_out_ids = nullptr;
-    uint8_t* d_out_status = nullptr; uint8_t* d_out_has = nullptr; uint32_t* d_out_len = nullptr;
-    SlowItem* d_slow = nullptr;                 // identity: work list of deferred tasks (kernel tail)
+    DevPtr<uint8_t> d_out_payload; DevPtr<uint64_t> d_out_off; DevPtr<uint4> d_out_ids;
+    DevPtr<uint8_t> d_out_status; DevPtr<uint8_t> d_out_has; DevPtr<uint32_t> d_out_len;
+    DevPtr<SlowItem> d_slow;                    // identity: work list of deferred tasks (kernel tail)
     uint32_t drain_epoch = 0;                   // tag of the current launch's work-list items
-    WireEnv* d_wire_env = nullptr;
-    uint32_t* d_crc_shift = nullptr;            // crc32: zero-byte shift tables
+    DevPtr<WireEnv> d_wire_env;
+    DevPtr<uint32_t> d_crc_shift;               // crc32: zero-byte shift tables
     uint64_t cancelled_pending = 0;            // pending tasks carrying B9_TF_CANCELLED (pushed so, expired, or b9_cancel)
-    CancelKey* d_cancel_keys = nullptr; uint32_t* d_cancel_out = nullptr; uint32_t cancel_cap = 0;   // b9_cancel: sorted ids + outcome words, grow-only
-    DrainCtl* d_ctl = nullptr; uint64_t* d_tile_state = nullptr;   // d_ctl: D3_CTL_RING control blocks (drain_kernel.cuh)
+    GrowBuf<CancelKey> d_cancel_keys; GrowBuf<uint32_t> d_cancel_out;   // b9_cancel: sorted ids + outcome words
+    DevPtr<DrainCtl> d_ctl; DevPtr<uint64_t> d_tile_state;   // d_ctl: D3_CTL_RING control blocks (drain_kernel.cuh)
     bool ctl_dirty = false;                    // the next drain's control block may be non-zero: zero the ring before it
     uint32_t ctl_last = 0;                     // control block of the last drain launch (read by finish_launch)
     bool last_op_drain = false;                // the drain stream's last operation is a drain3_kernel: the next may overlap it
     // launches since the last completion are timed as one span: ev_burst before the first one's kernel, ev_b right after
     // the last one's (recorded before anything else is enqueued on the drain stream, see end_drain_span)
-    bool burst_open = false; cudaEvent_t ev_burst = nullptr;
-    bool res_async = false;                    // the last launch returned before its kernels finished: finalize on fetch / sync
-    uint32_t res_async_n = 0; uint64_t res_async_in_bytes = 0;
-    DrainCtl* h_ctl = nullptr;                 // pinned
-    uint8_t* d_xchg_send = nullptr; uint8_t* d_xchg_recv = nullptr; uint64_t xchg_send_cap = 0, xchg_recv_cap = 0;   // b9_rebalance staging, grow-only
-    uint64_t* d_prefix = nullptr; unsigned long long* d_scan_sums = nullptr;   // b9_rebalance: byte prefix of the pending tasks, on the device
-    uint64_t* d_rtab = nullptr; uint64_t* h_rtab = nullptr; size_t rtab_words = 0;   // b9_rebalance: all-gather tables + cut points (device / pinned), allocated once
-    unsigned long long* d_count = nullptr; unsigned long long* h_count = nullptr;
-    // results waiting on the device for b9_drain_fetch
-    bool have_results = false, res_peek = false;
-    bool res_retry = false;                    // the waiting results come from a drain launched under a retry policy
-    bool res_cb = false, res_cb_keyed = false; int64_t res_cb_ts = 0;   // ... with a callback pass: its keying and Unix seconds
+    bool burst_open = false; Event ev_burst;
+    PinnedPtr<DrainCtl> h_ctl;
+    GrowBuf<uint8_t> d_xchg_send, d_xchg_recv; // b9_rebalance staging
+    DevPtr<uint64_t> d_prefix; DevPtr<unsigned long long> d_scan_sums;   // b9_rebalance: byte prefix of the pending tasks, on the device
+    DevPtr<uint64_t> d_rtab; PinnedPtr<uint64_t> h_rtab; size_t rtab_words = 0;   // b9_rebalance: all-gather tables + cut points (device / pinned), allocated once
+    DevPtr<unsigned long long> d_count; PinnedPtr<unsigned long long> h_count;
+    WaitingResults res;
     uint64_t res_gen = 0;                      // bumped whenever the waiting results change (launch, fetch commit)
-    uint32_t res_n = 0, res_popped = 0; uint64_t res_bytes = 0, res_in_bytes = 0; float res_kernel_ms = 0.f;
-    bool res_ids_in_ring = false; uint64_t res_head = 0;   // record j's id is the ring id of task res_head + j (DrainOut::ids_compacted == 0)
     bool expired_since_launch = false, recount_cancelled = false;   // (b9_expire between a launch and its fetch: recount, see b9_drain_fetch)
 
     // ---- multi-GPU (NCCL, loaded with dlopen: the library has no link-time dependency on it)
     void* nccl_comm = nullptr; int comm_rank = 0, comm_world = 1;
 
     b9_stats stats{};
+
+    // what the members do not release themselves: the segment events and the submission arenas' page-locked memory
+    // (submit_buffer.h builds without CUDA)
+    ~b9_ctx() {
+        for (const Segment& sg : segs) cudaEventDestroy(sg.ready);
+        for (cudaEvent_t e : event_pool) cudaEventDestroy(e);
+        if (sb) for (SubmitArena& A : sb->arena) {
+            if (A.payload) cudaFreeHost(A.payload);
+            if (A.offsets) cudaFreeHost(A.offsets);
+            if (A.ids) cudaFreeHost(A.ids);
+            if (A.flags) cudaFreeHost(A.flags);
+        }
+    }
 };
 
 namespace {
 
+// A `ready` event for a new segment: an idle one of the pool, else a new one. Caller holds c->mu.
+cudaError_t take_event(b9_ctx* c, cudaEvent_t* out) {
+    if (c->event_pool.empty()) return cudaEventCreateWithFlags(out, cudaEventDisableTiming);
+    *out = c->event_pool.back();
+    c->event_pool.pop_back();
+    return cudaSuccess;
+}
+
+// Gives a segment's `ready` event back to the pool. Caller holds c->mu.
+void put_event(b9_ctx* c, cudaEvent_t e) { c->event_pool.push_back(e); }
+
+// Appends a batch of n tasks at the tail as a new segment: ring bytes [start, start + bytes), its slots written by the work
+// `ready` was recorded behind. max_len: its longest task (0: not known); n_pickle: its tasks carrying B9_TF_PICKLE. The next
+// segment goes behind it, at most at `end` (the end of the free range it was placed in: the re-push fills ranges exactly,
+// b9_ring_free_ranges). Caller holds c->mu.
+void append_segment(b9_ctx* c, uint32_t n, uint64_t start, uint64_t bytes, uint32_t max_len, uint32_t n_pickle, cudaEvent_t ready,
+                    uint64_t end = UINT64_MAX) {
+    c->segs.push_back(Segment{c->tail_task, n, start, bytes, ready, max_len, n_pickle});
+    c->write_pos = std::min<uint64_t>(start + b9_seg_span(bytes), end);
+    c->tail_task += n;
+    c->pending_bytes += bytes;
+}
+
+// Frees the segments the head has moved past. Caller holds c->mu.
 void free_segments(b9_ctx* c) {
     while (!c->segs.empty() && c->segs.front().first_task + c->segs.front().n <= c->head_task) {
-        c->event_pool.push_back(c->segs.front().ready);
+        put_event(c, c->segs.front().ready);
         c->segs.pop_front();
     }
     if (c->segs.empty()) c->write_pos = 0;
+}
+
+// Makes stream s wait until every pending task is on the device (each live segment's `ready`). Caller holds c->mu.
+int wait_pending(const b9_ctx* c, cudaStream_t s) {
+    for (const Segment& sg : c->segs) CU(cudaStreamWaitEvent(s, sg.ready, 0));
+    return B9_OK;
+}
+
+// Copies the ids of the n tasks from `first_task` on between their ring slots and the linear buffer `buf` (16 bytes per id),
+// in two pieces when the slots wrap the ring. to_ring: buf -> slots, else slots -> buf; kind as for cudaMemcpyAsync.
+cudaError_t copy_slot_ids(const b9_ctx* c, uint64_t first_task, size_t n, const void* buf, bool to_ring, cudaMemcpyKind kind, cudaStream_t s) {
+    const uint32_t slot0 = (uint32_t)(first_task & c->slot_mask);
+    const size_t first = std::min<size_t>(n, (size_t)c->ring_tasks - slot0);
+    auto copy = [&](uint4* slots, const uint8_t* lin, size_t k) {
+        return to_ring ? cudaMemcpyAsync(slots, lin, k * 16, kind, s) : cudaMemcpyAsync((void*)lin, slots, k * 16, kind, s);
+    };
+    const cudaError_t e = copy(c->d_ids + slot0, (const uint8_t*)buf, first);
+    if (e != cudaSuccess || first == n) return e;
+    return copy(c->d_ids, (const uint8_t*)buf + first * 16, n - first);
 }
 
 // Closes the timed span of the drain launches enqueued so far (ev_b right behind the last drain kernel), before anything
@@ -387,24 +489,32 @@ __global__ void count_cancelled_kernel(const uint64_t* __restrict__ hdr, uint32_
     if ((threadIdx.x & 31u) == 0u && m) atomicAdd(count, (unsigned long long)__popc(m));
 }
 
-// cancelled_pending := the cancelled slots among the pending tasks, counted on the device. Caller holds c->out_mu (not c->mu).
-int recount_cancelled_locked_out(b9_ctx* c) {
-    uint64_t head = 0, depth = 0;
-    cudaStream_t s = c->stream;
-    {
-        std::lock_guard<std::mutex> lk(c->mu);
-        head = c->head_task; depth = c->tail_task - c->head_task;
-        for (const Segment& sg : c->segs) CU(cudaStreamWaitEvent(s, sg.ready, 0));
-    }
+// *out := the cancelled slots among tasks [head, head + depth), counted on stream s, which already waits for them. One kernel
+// when depth > 0 (the caller counts it); synchronises s. Caller holds c->out_mu (d_count and h_count are the drain side's).
+int count_cancelled(b9_ctx* c, uint64_t head, uint64_t depth, cudaStream_t s, uint64_t* out) {
     CU(cudaMemsetAsync(c->d_count, 0, sizeof(unsigned long long), s));
     if (depth) { count_cancelled_kernel<<<(uint32_t)((depth + 255) / 256), 256, 0, s>>>(c->d_hdr, c->slot_mask, head, (uint32_t)depth, c->d_count); CU(cudaGetLastError()); }
     CU(cudaMemcpyAsync(c->h_count, c->d_count, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
+    *out = *c->h_count;
+    return B9_OK;
+}
+
+// cancelled_pending := the cancelled slots among the pending tasks, counted on the device. Caller holds c->out_mu (not c->mu).
+int recount_cancelled_locked_out(b9_ctx* c) {
+    uint64_t head = 0, depth = 0, count = 0;
+    cudaStream_t s = c->stream;
+    {
+        std::lock_guard<std::mutex> lk(c->mu);
+        head = c->head_task; depth = c->tail_task - c->head_task;
+        if (const int rc = wait_pending(c, s)) return rc;
+    }
+    { const int rc = count_cancelled(c, head, depth, s, &count); if (rc) return rc; }
     std::lock_guard<std::mutex> lk(c->mu);
     // tasks pushed (with B9_TF_CANCELLED) after the snapshot are in cancelled_pending already but not in the count: keep them
     const uint64_t depth_now = c->tail_task - c->head_task;
-    if (depth_now == depth) c->cancelled_pending = *c->h_count;
-    else c->cancelled_pending = std::max<uint64_t>(c->cancelled_pending, *c->h_count);   // (an over-count only costs the count pre-pass)
+    if (depth_now == depth) c->cancelled_pending = count;
+    else c->cancelled_pending = std::max<uint64_t>(c->cancelled_pending, count);   // (an over-count only costs the count pre-pass)
     c->recount_cancelled = false;
     if (depth) c->stats.kernel_launches++;
     return B9_OK;
@@ -412,8 +522,8 @@ int recount_cancelled_locked_out(b9_ctx* c) {
 
 // Commits the pop of the fetched window (the head moves past it, its fully consumed segments are freed). Caller holds c->mu.
 void commit_pop(b9_ctx* c) {
-    c->head_task += c->res_popped; c->pending_bytes -= c->res_in_bytes; c->stats.tasks_drained += c->res_popped;
-    c->cancelled_pending -= std::min<uint64_t>(c->cancelled_pending, (uint64_t)(c->res_popped - c->res_n));
+    c->head_task += c->res.popped; c->pending_bytes -= c->res.in_bytes; c->stats.tasks_drained += c->res.popped;
+    c->cancelled_pending -= std::min<uint64_t>(c->cancelled_pending, (uint64_t)(c->res.popped - c->res.n));
     c->recount_cancelled = c->expired_since_launch;              // an expire ran between this drain's launch and its commit: its
                                                                   // count included tasks of the window that are gone now
     free_segments(c);
@@ -456,21 +566,12 @@ __global__ void retry_gather_kernel(const uint32_t* __restrict__ rec, uint32_t n
 int commit_with_repush(b9_ctx* c, const std::vector<uint32_t>& retry_rec, float d2h_ms, uint64_t d2h_bytes) {
     const uint32_t k = (uint32_t)retry_rec.size();
     cudaStream_t s = c->stream_in;
-    const uint64_t head = c->res_head;
-    if (c->retry_bytes_cap < c->res_in_bytes) {                            // (the retried bytes are at most the window's)
-        cudaFree(c->d_retry_bytes); c->d_retry_bytes = nullptr; c->retry_bytes_cap = 0;
-        const cudaError_t e = cudaMalloc(&c->d_retry_bytes, c->res_in_bytes + RING_SLACK);
-        if (e != cudaSuccess) { cudaGetLastError(); return fail(B9_ENOMEM, "b9_drain_fetch: %llu bytes of re-push scratch: %s", (unsigned long long)c->res_in_bytes, cudaGetErrorString(e)); }
-        c->retry_bytes_cap = c->res_in_bytes;
-    }
+    const uint64_t head = c->res.head;
+    // (the retried bytes are at most the window's)
+    { const int rc = c->d_retry_bytes.ensure(c->res.in_bytes + RING_SLACK, "b9_drain_fetch: re-push scratch"); if (rc) return rc; }
     size_t scan_bytes = 0;
     CU(cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, c->d_in_off + 1, c->d_in_off + 1, (int)k, s));
-    if (c->retry_scan_cap < scan_bytes) {
-        cudaFree(c->d_retry_scan); c->d_retry_scan = nullptr; c->retry_scan_cap = 0;
-        const cudaError_t e = cudaMalloc(&c->d_retry_scan, scan_bytes);
-        if (e != cudaSuccess) { cudaGetLastError(); return fail(B9_ENOMEM, "b9_drain_fetch: re-push scan scratch: %s", cudaGetErrorString(e)); }
-        c->retry_scan_cap = scan_bytes;
-    }
+    { const int rc = c->d_retry_scan.ensure(scan_bytes, "b9_drain_fetch: re-push scan scratch"); if (rc) return rc; }
     const int64_t now = (int64_t)std::chrono::duration_cast<std::chrono::seconds>(std::chrono::system_clock::now().time_since_epoch()).count();
     CU(cudaMemcpyAsync(c->d_retry_rec, retry_rec.data(), (size_t)k * 4, cudaMemcpyHostToDevice, s));
     retry_len_kernel<<<(k + 255) / 256, 256, 0, s>>>(c->d_retry_rec, k, c->d_task_of, c->d_hdr, head, c->slot_mask, c->d_in_off);
@@ -486,7 +587,7 @@ int commit_with_repush(b9_ctx* c, const std::vector<uint32_t>& retry_rec, float 
     // a segment it ends inside is trimmed to start at the first task behind the window (its offset is read back here), so
     // that the window's bytes are free wherever they lie. The ring's free ranges then hold the retried bytes, which are at
     // most the window's: they are placed in range order as one segment, or two when the freed bytes straddle the ring's end.
-    const uint64_t new_head = c->head_task + c->res_popped;               // (only drain-side calls move the head: out_mu is held)
+    const uint64_t new_head = c->head_task + c->res.popped;               // (only drain-side calls move the head: out_mu is held)
     Segment part{}; bool partial = false;
     {
         std::lock_guard<std::mutex> lk(c->mu);
@@ -534,9 +635,8 @@ int commit_with_repush(b9_ctx* c, const std::vector<uint32_t>& retry_rec, float 
     cudaEvent_t ready[2] = {nullptr, nullptr};
     {
         std::lock_guard<std::mutex> lk(c->mu);
-        for (int q = 0; q < n_plan && !c->event_pool.empty(); ++q) { ready[q] = c->event_pool.back(); c->event_pool.pop_back(); }
+        for (int q = 0; q < n_plan; ++q) CU(take_event(c, &ready[q]));
     }
-    for (int q = 0; q < n_plan; ++q) if (!ready[q]) CU(cudaEventCreateWithFlags(&ready[q], cudaEventDisableTiming));
     std::lock_guard<std::mutex> lk(c->mu);
     c->stats.last_drain_d2h_ms = d2h_ms;
     c->stats.bytes_d2h += d2h_bytes;
@@ -550,10 +650,7 @@ int commit_with_repush(b9_ctx* c, const std::vector<uint32_t>& retry_rec, float 
             }
     const uint64_t tail = c->tail_task;
     // (enqueue only: nothing here waits for the device)
-    const uint32_t slot0 = (uint32_t)(tail & c->slot_mask);
-    const uint32_t first = std::min<uint32_t>(k, c->ring_tasks - slot0);
-    CU(cudaMemcpyAsync(c->d_ids + slot0, c->d_retry_ids, (size_t)first * 16, cudaMemcpyDeviceToDevice, s));
-    if (first < k) CU(cudaMemcpyAsync(c->d_ids, c->d_retry_ids + first, (size_t)(k - first) * 16, cudaMemcpyDeviceToDevice, s));
+    CU(copy_slot_ids(c, tail, k, c->d_retry_ids, true, cudaMemcpyDeviceToDevice, s));
     for (int q = 0; q < n_plan; ++q) {
         const Piece& pc = plan[q];
         const uint32_t n = pc.i1 - pc.i0;
@@ -563,11 +660,8 @@ int commit_with_repush(b9_ctx* c, const std::vector<uint32_t>& retry_rec, float 
                                                       c->d_off, c->d_hdr, c->d_ts, c->d_exp);
         CU(cudaGetLastError());
         CU(cudaEventRecord(ready[q], s));
-        c->segs.push_back(Segment{tail + pc.i0, n, pc.at, pc.hi - pc.lo, ready[q], 0u});
-        c->write_pos = std::min<uint64_t>(pc.at + b9_seg_span(pc.hi - pc.lo), pc.end);
+        append_segment(c, n, pc.at, pc.hi - pc.lo, 0u, 0u, ready[q], pc.end);   // (no B9_TF_PICKLE task gets a RETRY record)
     }
-    c->tail_task += k;
-    c->pending_bytes += bytes;
     c->stats.kernel_launches += 3 + (uint64_t)n_plan;                      // (length, the scan, gather, ingest per segment)
     return B9_OK;
 }
@@ -583,18 +677,13 @@ int b9_set_retry_policy(b9_ctx* c, uint32_t exc_mask, uint32_t max_retries) {
     if (exc_mask & ~B9_EXC_ALL) return fail(B9_EINVAL, "b9_set_retry_policy: exception bits 0x%x are not B9_EXC_*", exc_mask & ~B9_EXC_ALL);
     if (max_retries > 255) return fail(B9_EINVAL, "b9_set_retry_policy: max_retries %u: a task's retries are one byte (b9_push_meta.retries)", max_retries);
     OutLock out_lk(c);
-    if (exc_mask && !c->d_task_of) {
+    if (exc_mask) {
         CU(cudaSetDevice(c->device));
-        const size_t md = c->max_drain_tasks;
-        cudaError_t e = cudaMalloc(&c->d_task_of, md * sizeof(uint32_t));
-        if (e == cudaSuccess) e = cudaMalloc(&c->d_retry_rec, md * sizeof(uint32_t));
-        if (e == cudaSuccess) e = cudaMalloc(&c->d_retry_ids, md * sizeof(uint4));
-        if (e != cudaSuccess) {
-            cudaGetLastError();
-            cudaFree(c->d_task_of); cudaFree(c->d_retry_rec); cudaFree(c->d_retry_ids);
-            c->d_task_of = nullptr; c->d_retry_rec = nullptr; c->d_retry_ids = nullptr;
-            return fail(e == cudaErrorMemoryAllocation ? B9_ENOMEM : B9_EIO, "b9_set_retry_policy: %s", cudaGetErrorString(e));
-        }
+        const uint64_t md = c->max_drain_tasks;
+        int rc = c->d_task_of.ensure(md * sizeof(uint32_t), "b9_set_retry_policy: task_of");
+        if (rc == B9_OK) rc = c->d_retry_rec.ensure(md * sizeof(uint32_t), "b9_set_retry_policy: retry records");
+        if (rc == B9_OK) rc = c->d_retry_ids.ensure(md * sizeof(uint4), "b9_set_retry_policy: retry ids");
+        if (rc) return rc;
     }
     c->retry_mask = exc_mask;
     c->max_retries = max_retries;
@@ -605,17 +694,12 @@ int b9_set_callback_policy(b9_ctx* c, int enabled, const uint8_t* signing_key, u
     if (!c) return fail(B9_EINVAL, "b9_set_callback_policy: ctx is NULL");
     if (enabled && key_len && !signing_key) return fail(B9_EINVAL, "b9_set_callback_policy: NULL signing_key with key_len %u", key_len);
     OutLock out_lk(c);
-    if (enabled && !c->d_cb_kind) {
+    if (enabled) {
         CU(cudaSetDevice(c->device));
-        const size_t md = c->max_drain_tasks;
-        cudaError_t e = cudaMalloc(&c->d_cb_kind, md);
-        if (e == cudaSuccess) e = cudaMalloc(&c->d_cb_digest, md * 32);
-        if (e != cudaSuccess) {
-            cudaGetLastError();
-            cudaFree(c->d_cb_kind); cudaFree(c->d_cb_digest);
-            c->d_cb_kind = nullptr; c->d_cb_digest = nullptr;
-            return fail(e == cudaErrorMemoryAllocation ? B9_ENOMEM : B9_EIO, "b9_set_callback_policy: %s", cudaGetErrorString(e));
-        }
+        const uint64_t md = c->max_drain_tasks;
+        int rc = c->d_cb_kind.ensure(md, "b9_set_callback_policy: callback kinds");
+        if (rc == B9_OK) rc = c->d_cb_digest.ensure(md * 32, "b9_set_callback_policy: digests");
+        if (rc) return rc;
     }
     c->cb_enabled = enabled != 0;
     c->cb_keyed = c->cb_enabled && key_len != 0;
@@ -672,33 +756,33 @@ int b9_ctx_create(const b9_opts* opts, b9_ctx** out) {
     cudaDeviceProp prop{};
     CUC(cudaGetDeviceProperties(&prop, c->device));
     c->sm_count = prop.multiProcessorCount;
-    CUC(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
-    CUC(cudaStreamCreateWithFlags(&c->stream_in, cudaStreamNonBlocking));
-    CUC(cudaEventCreate(&c->ev_burst));
-    CUC(cudaEventCreate(&c->ev_a)); CUC(cudaEventCreate(&c->ev_b)); CUC(cudaEventCreate(&c->ev_c)); CUC(cudaEventCreate(&c->ev_d));
-    CUC(cudaEventCreate(&c->ev_pa)); CUC(cudaEventCreate(&c->ev_pb));
+    CUC(cudaStreamCreateWithFlags(&c->stream.v, cudaStreamNonBlocking));
+    CUC(cudaStreamCreateWithFlags(&c->stream_in.v, cudaStreamNonBlocking));
+    CUC(cudaEventCreate(&c->ev_burst.v));
+    CUC(cudaEventCreate(&c->ev_a.v)); CUC(cudaEventCreate(&c->ev_b.v)); CUC(cudaEventCreate(&c->ev_c.v)); CUC(cudaEventCreate(&c->ev_d.v));
+    CUC(cudaEventCreate(&c->ev_pa.v)); CUC(cudaEventCreate(&c->ev_pb.v));
     const uint32_t rt = c->ring_tasks, md = c->max_drain_tasks;
-    CUC(cudaMalloc(&c->d_payload, c->ring_bytes + RING_SLACK));
+    CUC(cudaMalloc(&c->d_payload.v, c->ring_bytes + RING_SLACK));
     CUC(cudaMemset(c->d_payload + c->ring_bytes, 0, RING_SLACK));
-    CUC(cudaMalloc(&c->d_off, rt * sizeof(uint64_t)));
-    CUC(cudaMalloc(&c->d_hdr, rt * sizeof(uint64_t)));
-    CUC(cudaMalloc(&c->d_ids, rt * sizeof(uint4)));
-    CUC(cudaMalloc(&c->d_ts, rt * sizeof(int64_t)));
-    CUC(cudaMalloc(&c->d_exp, rt * sizeof(int64_t)));
-    CUC(cudaMalloc(&c->d_in_off, ((size_t)rt + 1) * sizeof(uint64_t)));
-    CUC(cudaMalloc(&c->d_in_ts, rt * sizeof(int64_t)));
-    CUC(cudaMalloc(&c->d_in_exp, rt * sizeof(int64_t)));
-    CUC(cudaMalloc(&c->d_in_retries, rt));
-    CUC(cudaMalloc(&c->d_in_flags, rt));
-    CUC(cudaMalloc(&c->d_out_payload, c->max_result_bytes + RING_SLACK));
-    CUC(cudaMalloc(&c->d_out_off, ((size_t)md + 1) * sizeof(uint64_t)));
-    CUC(cudaMalloc(&c->d_out_ids, (size_t)md * sizeof(uint4)));
-    CUC(cudaMalloc(&c->d_out_status, md));
-    CUC(cudaMalloc(&c->d_out_has, md));
-    CUC(cudaMalloc(&c->d_out_len, (size_t)md * sizeof(uint32_t)));
-    CUC(cudaMalloc(&c->d_slow, (size_t)md * sizeof(SlowItem)));
+    CUC(cudaMalloc(&c->d_off.v, rt * sizeof(uint64_t)));
+    CUC(cudaMalloc(&c->d_hdr.v, rt * sizeof(uint64_t)));
+    CUC(cudaMalloc(&c->d_ids.v, rt * sizeof(uint4)));
+    CUC(cudaMalloc(&c->d_ts.v, rt * sizeof(int64_t)));
+    CUC(cudaMalloc(&c->d_exp.v, rt * sizeof(int64_t)));
+    CUC(cudaMalloc(&c->d_in_off.v, ((size_t)rt + 1) * sizeof(uint64_t)));
+    CUC(cudaMalloc(&c->d_in_ts.v, rt * sizeof(int64_t)));
+    CUC(cudaMalloc(&c->d_in_exp.v, rt * sizeof(int64_t)));
+    CUC(cudaMalloc(&c->d_in_retries.v, rt));
+    CUC(cudaMalloc(&c->d_in_flags.v, rt));
+    CUC(cudaMalloc(&c->d_out_payload.v, c->max_result_bytes + RING_SLACK));
+    CUC(cudaMalloc(&c->d_out_off.v, ((size_t)md + 1) * sizeof(uint64_t)));
+    CUC(cudaMalloc(&c->d_out_ids.v, (size_t)md * sizeof(uint4)));
+    CUC(cudaMalloc(&c->d_out_status.v, md));
+    CUC(cudaMalloc(&c->d_out_has.v, md));
+    CUC(cudaMalloc(&c->d_out_len.v, (size_t)md * sizeof(uint32_t)));
+    CUC(cudaMalloc(&c->d_slow.v, (size_t)md * sizeof(SlowItem)));
     CUC(cudaMemset(c->d_slow, 0, (size_t)md * sizeof(SlowItem)));
-    CUC(cudaMalloc(&c->d_wire_env, sizeof(WireEnv)));
+    CUC(cudaMalloc(&c->d_wire_env.v, sizeof(WireEnv)));
     {
         // Z_k = advance the reflected CRC-32 register over 2^k zero bytes, as 4 byte-indexed tables per k
         std::vector<uint32_t> tabs((size_t)CRC_SHIFT_LEVELS * 1024);
@@ -710,15 +794,15 @@ int b9_ctx_create(const b9_opts* opts, b9_ctx** out) {
             const uint32_t* prev = tabs.data() + (size_t)(k - 1) * 1024; uint32_t* cur = tabs.data() + (size_t)k * 1024;
             for (uint32_t j = 0; j < 4; ++j) for (uint32_t b = 0; b < 256; ++b) cur[j * 256 + b] = apply(prev, apply(prev, b << (8 * j)));
         }
-        CUC(cudaMalloc(&c->d_crc_shift, tabs.size() * sizeof(uint32_t)));
+        CUC(cudaMalloc(&c->d_crc_shift.v, tabs.size() * sizeof(uint32_t)));
         CUC(cudaMemcpy(c->d_crc_shift, tabs.data(), tabs.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
     }
-    CUC(cudaMalloc(&c->d_ctl, D3_CTL_RING * sizeof(DrainCtl)));
+    CUC(cudaMalloc(&c->d_ctl.v, D3_CTL_RING * sizeof(DrainCtl)));
     CUC(cudaMemset(c->d_ctl, 0, D3_CTL_RING * sizeof(DrainCtl)));
-    CUC(cudaMalloc(&c->d_tile_state, ((size_t)md / D2_THREADS + 2) * sizeof(uint64_t)));
-    CUC(cudaMalloc(&c->d_count, sizeof(unsigned long long)));
-    CUC(cudaHostAlloc(&c->h_ctl, sizeof(DrainCtl), cudaHostAllocDefault));
-    CUC(cudaHostAlloc(&c->h_count, sizeof(unsigned long long), cudaHostAllocDefault));
+    CUC(cudaMalloc(&c->d_tile_state.v, ((size_t)md / D2_THREADS + 2) * sizeof(uint64_t)));
+    CUC(cudaMalloc(&c->d_count.v, sizeof(unsigned long long)));
+    CUC(cudaHostAlloc(&c->h_ctl.v, sizeof(DrainCtl), cudaHostAllocDefault));
+    CUC(cudaHostAlloc(&c->h_count.v, sizeof(unsigned long long), cudaHostAllocDefault));
     c->stats.sm_count = (uint32_t)c->sm_count;
     if (const char* v = getenv("B9_STAGE_BYTES")) c->stage_bytes_override = ((uint32_t)atoi(v) + 1023u) & ~1023u;
 #undef CUC
@@ -732,48 +816,7 @@ void b9_ctx_destroy(b9_ctx* c) {
     if (c->stream) cudaStreamSynchronize(c->stream);
     if (c->stream_in) cudaStreamSynchronize(c->stream_in);
     if (c->nccl_comm) nccl_comm_destroy(c->nccl_comm);
-    for (Segment& sg : c->segs) cudaEventDestroy(sg.ready);
-    for (cudaEvent_t e : c->event_pool) cudaEventDestroy(e);
-    cudaFree(c->d_payload); cudaFree(c->d_off); cudaFree(c->d_hdr); cudaFree(c->d_ids); cudaFree(c->d_ts); cudaFree(c->d_exp);
-    cudaFree(c->d_in_off); cudaFree(c->d_in_ts); cudaFree(c->d_in_exp); cudaFree(c->d_in_retries); cudaFree(c->d_in_flags);
-    cudaFree(c->d_out_payload); cudaFree(c->d_out_off); cudaFree(c->d_out_ids); cudaFree(c->d_out_status); cudaFree(c->d_out_has); cudaFree(c->d_out_len); cudaFree(c->d_slow); cudaFree(c->d_wire_env); cudaFree(c->d_crc_shift);
-    cudaFree(c->d_ctl); cudaFree(c->d_tile_state); cudaFree(c->d_count);
-    cudaFree(c->d_cancel_keys); cudaFree(c->d_cancel_out);
-    cudaFree(c->d_task_of); cudaFree(c->d_retry_rec); cudaFree(c->d_retry_ids); cudaFree(c->d_retry_bytes); cudaFree(c->d_retry_scan);
-    cudaFree(c->d_cb_kind); cudaFree(c->d_cb_digest);
-    if (c->h_ctl) cudaFreeHost(c->h_ctl);
-    if (c->h_rtab) cudaFreeHost(c->h_rtab);
-    cudaFree(c->d_rtab); cudaFree(c->d_prefix); cudaFree(c->d_scan_sums);
-    cudaFree(c->d_xchg_send); cudaFree(c->d_xchg_recv);
-    if (c->h_count) cudaFreeHost(c->h_count);
-    if (c->ev_burst) cudaEventDestroy(c->ev_burst);
-    if (c->ev_a) cudaEventDestroy(c->ev_a);
-    if (c->ev_b) cudaEventDestroy(c->ev_b);
-    if (c->ev_c) cudaEventDestroy(c->ev_c);
-    if (c->ev_d) cudaEventDestroy(c->ev_d);
-    if (c->ev_pa) cudaEventDestroy(c->ev_pa);
-    if (c->ev_pb) cudaEventDestroy(c->ev_pb);
-    delete c->pack_pool;
-    if (c->sb) {
-        for (int k = 0; k < 2; ++k) {
-            SubmitArena& A = c->sb->arena[k];
-            if (A.payload) cudaFreeHost(A.payload);
-            if (A.offsets) cudaFreeHost(A.offsets);
-            if (A.ids) cudaFreeHost(A.ids);
-            if (A.flags) cudaFreeHost(A.flags);
-            if (c->sb_free[k]) cudaEventDestroy(c->sb_free[k]);
-        }
-        delete c->sb;
-    }
-    for (PackArena& A : c->pack) {
-        if (A.payload) cudaFreeHost(A.payload);
-        if (A.offsets) cudaFreeHost(A.offsets);
-        if (A.ids) cudaFreeHost(A.ids);
-        if (A.free_ev) cudaEventDestroy(A.free_ev);
-    }
-    if (c->stream) cudaStreamDestroy(c->stream);
-    if (c->stream_in) cudaStreamDestroy(c->stream_in);
-    delete c;
+    delete c;                                   // (its members release the device memory, pinned memory, events and streams)
 }
 
 void* b9_host_alloc(b9_ctx* c, uint64_t bytes) {
@@ -815,11 +858,9 @@ static int push_impl(b9_ctx* c, const uint8_t* task_ids, const uint8_t* payload,
         if (!place_segment(c, bytes, &start))
             return fail(B9_ENOSPC, "b9_batch_push: %llu payload bytes do not fit the ring (%llu pending of %llu)",
                         (unsigned long long)bytes, (unsigned long long)c->pending_bytes, (unsigned long long)c->ring_bytes);
-        if (!c->event_pool.empty()) { ready = c->event_pool.back(); c->event_pool.pop_back(); }
+        CU(take_event(c, &ready));
         tail = c->tail_task;
     }
-    if (!ready) CU(cudaEventCreateWithFlags(&ready, cudaEventDisableTiming));
-    auto give_back = [&]() { std::lock_guard<std::mutex> lk(c->mu); c->event_pool.push_back(ready); };
     cudaStream_t s = c->stream_in;
     CU(cudaEventRecord(c->ev_pa, s));
     // the payload DMA goes first (into ring space that stays free until this push is committed), so that
@@ -838,7 +879,7 @@ static int push_impl(b9_ctx* c, const uint8_t* task_ids, const uint8_t* payload,
         }
         seg_max_len = (uint32_t)std::min<uint64_t>(longest, maxb);
         if (bad != ~0ull || big != ~0ull) {
-            give_back();
+            { std::lock_guard<std::mutex> lk(c->mu); put_event(c, ready); }
             cudaStreamSynchronize(s);            // the stray DMA must not outlive the caller's buffer
             if (bad != ~0ull) return fail(B9_EINVAL, "b9_batch_push: offsets not monotonic at task %llu", (unsigned long long)bad);
             return fail(B9_E2BIG, "b9_batch_push: task %llu is %llu bytes, max_task_bytes is %u", (unsigned long long)big,
@@ -850,11 +891,7 @@ static int push_impl(b9_ctx* c, const uint8_t* task_ids, const uint8_t* payload,
         }
     }
     CU(cudaMemcpyAsync(c->d_in_off, offsets, ((size_t)n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
-    // ids go straight into their ring slots (two pieces when the slot ring wraps)
-    const uint32_t slot0 = (uint32_t)(tail & c->slot_mask);
-    const uint32_t first = std::min<uint32_t>(n, c->ring_tasks - slot0);
-    CU(cudaMemcpyAsync(c->d_ids + slot0, task_ids, (size_t)first * 16, cudaMemcpyHostToDevice, s));
-    if (first < n) CU(cudaMemcpyAsync(c->d_ids, task_ids + (size_t)first * 16, (size_t)(n - first) * 16, cudaMemcpyHostToDevice, s));
+    CU(copy_slot_ids(c, tail, n, task_ids, true, cudaMemcpyHostToDevice, s));   // (ids go straight into their ring slots)
     const int64_t* ts = nullptr; const int64_t* ex = nullptr; const uint8_t* rt = nullptr; const uint8_t* fl = nullptr;
     uint64_t meta_bytes = 0;
     if (meta) {
@@ -871,11 +908,7 @@ static int push_impl(b9_ctx* c, const uint8_t* task_ids, const uint8_t* payload,
     CU(cudaEventRecord(ready, s));
     {
         std::lock_guard<std::mutex> lk(c->mu);
-        c->segs.push_back(Segment{tail, n, start, bytes, ready, seg_max_len});
-        c->segs.back().n_pickle = n_pickle;
-        c->write_pos = start + b9_seg_span(bytes);
-        c->tail_task += n;
-        c->pending_bytes += bytes;
+        append_segment(c, n, start, bytes, seg_max_len, n_pickle, ready);   // (tail_task == tail: in_mu is held)
         c->cancelled_pending += n_cancelled;
         c->stats.kernel_launches++;
         c->stats.tasks_pushed += n;
@@ -910,7 +943,7 @@ int b9_batch_push_v(b9_ctx* c, const uint8_t* task_ids, const uint8_t* const* pa
     if (!c->pack_pool) {
         int nt = (int)std::min<unsigned>(16u, std::max(1u, std::thread::hardware_concurrency()));
         if (const char* e = getenv("B9_PACK_THREADS")) nt = std::max(1, atoi(e));
-        c->pack_pool = new (std::nothrow) PackPool(nt);
+        c->pack_pool.reset(new (std::nothrow) PackPool(nt));
         if (!c->pack_pool) return fail(B9_ENOMEM, "b9_batch_push_v: thread pool");
     }
     const int T = c->pack_pool->nthreads;
@@ -927,23 +960,11 @@ int b9_batch_push_v(b9_ctx* c, const uint8_t* task_ids, const uint8_t* const* pa
     PackArena& A = c->pack[c->pack_next];
     c->pack_next ^= 1;
     if (A.in_flight) { CU(cudaEventSynchronize(A.free_ev)); A.in_flight = false; }   // its previous batch is on the device
-    if (!A.free_ev) CU(cudaEventCreateWithFlags(&A.free_ev, cudaEventDisableTiming));
-    if (A.cap_bytes < total + 64) {
-        if (A.payload) cudaFreeHost(A.payload);
-        A.payload = nullptr; A.cap_bytes = 0;
-        const uint64_t want = (total + 64) + (total + 64) / 4;
-        if (cudaHostAlloc(&A.payload, want, cudaHostAllocDefault) != cudaSuccess) { cudaGetLastError(); return fail(B9_ENOMEM, "b9_batch_push_v: %llu bytes of page-locked memory", (unsigned long long)want); }
-        A.cap_bytes = want;
-    }
-    if (A.cap_tasks < n) {
-        if (A.offsets) cudaFreeHost(A.offsets);
-        if (A.ids) cudaFreeHost(A.ids);
-        A.offsets = nullptr; A.ids = nullptr; A.cap_tasks = 0;
-        const uint32_t want = n + n / 4 + 16;
-        if (cudaHostAlloc(&A.offsets, ((size_t)want + 1) * 8, cudaHostAllocDefault) != cudaSuccess ||
-            cudaHostAlloc(&A.ids, (size_t)want * 16, cudaHostAllocDefault) != cudaSuccess) { cudaGetLastError(); return fail(B9_ENOMEM, "b9_batch_push_v: page-locked index"); }
-        A.cap_tasks = want;
-    }
+    if (!A.free_ev) CU(cudaEventCreateWithFlags(&A.free_ev.v, cudaEventDisableTiming));
+    // (room for a quarter more bytes, and a quarter + 16 more tasks)
+    { const int rc = A.payload.ensure(total + 64, "b9_batch_push_v: page-locked payload", (total + 64) / 4); if (rc) return rc; }
+    { const int rc = A.offsets.ensure(((uint64_t)n + 1) * 8, "b9_batch_push_v: page-locked offsets", ((uint64_t)n / 4 + 16) * 8); if (rc) return rc; }
+    { const int rc = A.ids.ensure((uint64_t)n * 16, "b9_batch_push_v: page-locked ids", ((uint64_t)n / 4 + 16) * 16); if (rc) return rc; }
     // pass 2: gather
     c->pack_pool->run([&](int t) {
         const uint32_t lo = lo_of(t), hi = lo_of(t + 1);
@@ -990,9 +1011,9 @@ static int sb_ensure(b9_ctx* c) {
             return fail(B9_ENOMEM, "b9_submit: %llu bytes of page-locked memory per arena", (unsigned long long)bytes);
         }
         A.cap_bytes = bytes; A.cap_tasks = tasks;
-        CU(cudaEventCreateWithFlags(&c->sb_free[k], cudaEventDisableTiming));
+        CU(cudaEventCreateWithFlags(&c->sb_free[k].v, cudaEventDisableTiming));
     }
-    c->sb = sb;
+    c->sb.reset(sb);
     return B9_OK;
 }
 
@@ -1008,7 +1029,7 @@ static int sb_push(b9_ctx* c, int k, uint32_t n) {
 int64_t b9_flush(b9_ctx* c) {
     if (!c) return fail(B9_EINVAL, "b9_flush: ctx is NULL");
     if (!c->sb) return 0;
-    SubmitBuffer* sb = c->sb;
+    SubmitBuffer* sb = c->sb.get();
     std::lock_guard<std::mutex> lk(sb->flush_mu);
     CU(cudaSetDevice(c->device));
     int64_t pushed = 0;
@@ -1073,7 +1094,7 @@ int64_t b9_expire(b9_ctx* c, int64_t now_unix_ns) {
         std::lock_guard<std::mutex> lk(c->mu);
         head = c->head_task; depth = c->tail_task - c->head_task;
         if (!depth) return 0;
-        for (const Segment& sg : c->segs) CU(cudaStreamWaitEvent(c->stream, sg.ready, 0));
+        if (const int rc = wait_pending(c, c->stream)) return rc;
     }
     CU(cudaMemsetAsync(c->d_count, 0, sizeof(unsigned long long), c->stream));
     expire_kernel<<<(uint32_t)((depth + 255) / 256), 256, 0, c->stream>>>(c->d_hdr, c->d_exp, c->slot_mask, head, (uint32_t)depth, now_unix_ns, c->d_count);
@@ -1108,17 +1129,11 @@ int64_t b9_cancel(b9_ctx* c, const uint8_t* task_ids, uint32_t n, uint8_t* outco
         std::lock_guard<std::mutex> lk(c->mu);
         head = c->head_task; depth = c->tail_task - c->head_task;
         if (!depth) return 0;
-        for (const Segment& sg : c->segs) CU(cudaStreamWaitEvent(s, sg.ready, 0));
+        if (const int rc = wait_pending(c, s)) return rc;
     }
     const uint32_t claimed = (uint32_t)std::min<uint64_t>(c->running.load(std::memory_order_relaxed), depth);   // (set and cleared under out_mu)
-    if (c->cancel_cap < n_keys) {
-        cudaFree(c->d_cancel_keys); cudaFree(c->d_cancel_out);
-        c->d_cancel_keys = nullptr; c->d_cancel_out = nullptr; c->cancel_cap = 0;
-        cudaError_t e = cudaMalloc(&c->d_cancel_keys, (size_t)n_keys * sizeof(CancelKey));
-        if (e == cudaSuccess) e = cudaMalloc(&c->d_cancel_out, (size_t)n_keys * sizeof(uint32_t));
-        if (e != cudaSuccess) { cudaGetLastError(); return fail(e == cudaErrorMemoryAllocation ? B9_ENOMEM : B9_EIO, "b9_cancel: %u keys: %s", n_keys, cudaGetErrorString(e)); }
-        c->cancel_cap = n_keys;
-    }
+    { const int rc = c->d_cancel_keys.ensure((uint64_t)n_keys * sizeof(CancelKey), "b9_cancel: keys"); if (rc) return rc; }
+    { const int rc = c->d_cancel_out.ensure((uint64_t)n_keys * sizeof(uint32_t), "b9_cancel: outcome words"); if (rc) return rc; }
     CU(cudaMemcpyAsync(c->d_cancel_keys, keys.data(), (size_t)n_keys * sizeof(CancelKey), cudaMemcpyHostToDevice, s));
     CU(cudaMemsetAsync(c->d_cancel_out, 0, (size_t)n_keys * sizeof(uint32_t), s));
     CU(cudaMemsetAsync(c->d_count, 0, sizeof(unsigned long long), s));
@@ -1143,28 +1158,28 @@ int64_t b9_cancel(b9_ctx* c, const uint8_t* task_ids, uint32_t n, uint8_t* outco
 
 // Waits for the last launch and publishes its outcome (records, bytes, overflow) to the ctx. Caller holds c->out_mu (not c->mu).
 static int finish_launch(b9_ctx* c) {
-    if (!c->res_async) return B9_OK;
-    c->res_async = false;
+    if (!c->res.async) return B9_OK;
+    c->res.async = false;
     end_drain_span(c);
     CU(cudaMemcpyAsync(c->h_ctl, c->d_ctl + c->ctl_last, sizeof(DrainCtl), cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
     // one launch: the time around its kernels; a burst of B9_DRAIN_ASYNC launches: from the first one's start to the last one's end
     float ms = 0; cudaEventElapsedTime(&ms, c->ev_burst, c->ev_b);
     c->burst_open = false;
-    c->res_kernel_ms = ms;
+    c->res.kernel_ms = ms;
     if (c->h_ctl->overflow) {
         c->running.store(0, std::memory_order_relaxed);
         return fail(B9_ENOSPC, "b9_drain_launch: results exceed max_result_bytes (%llu); drain fewer tasks or enlarge the staging",
                     (unsigned long long)c->max_result_bytes);
     }
-    c->res_bytes = c->h_ctl->bytes; c->res_n = c->h_ctl->total_cnt;
-    c->res_popped = c->res_async_n;
-    c->res_in_bytes = c->res_async_in_bytes;
-    c->have_results = true;
+    c->res.bytes = c->h_ctl->bytes; c->res.n = c->h_ctl->total_cnt;
+    c->res.popped = c->res.async_n;
+    c->res.in_bytes = c->res.async_in_bytes;
+    c->res.have = true;
     std::lock_guard<std::mutex> lk(c->mu);
     c->stats.last_drain_kernel_ms = ms;
-    c->stats.last_drain_in_bytes = c->res_async_in_bytes;
-    c->stats.last_drain_out_bytes = c->res_bytes;
+    c->stats.last_drain_in_bytes = c->res.async_in_bytes;
+    c->stats.last_drain_out_bytes = c->res.bytes;
     return B9_OK;
 }
 
@@ -1176,13 +1191,13 @@ static int64_t drain_launch_common(b9_ctx* c, int handler, uint32_t max_tasks, i
     CU(cudaSetDevice(c->device));
     // results of an earlier launch that were never fetched are dropped; their tasks are still
     // pending (a pop is committed by a successful fetch, never by a launch). (An open burst of async launches stays open.)
-    c->have_results = false; c->res_async = false;
+    c->res = WaitingResults{};
     c->running.store(0, std::memory_order_relaxed);
-    c->res_n = 0; c->res_popped = 0; c->res_bytes = 0; c->res_in_bytes = 0; c->res_peek = (peek & B9_DRAIN_PEEK) != 0;
-    c->res_gen++; c->res_retry = false;
+    c->res_gen++;
+    c->res.peek = (peek & B9_DRAIN_PEEK) != 0;
     // the callback pass signs with the host clock's Unix seconds, read once per launch (SignPayload's time.Now().Unix())
-    c->res_cb = !endpoint && c->cb_enabled; c->res_cb_keyed = c->res_cb && c->cb_keyed;
-    c->res_cb_ts = c->res_cb_keyed ? (int64_t)std::chrono::duration_cast<std::chrono::seconds>(std::chrono::system_clock::now().time_since_epoch()).count() : 0;
+    c->res.cb = !endpoint && c->cb_enabled; c->res.cb_keyed = c->res.cb && c->cb_keyed;
+    c->res.cb_ts = c->res.cb_keyed ? (int64_t)std::chrono::duration_cast<std::chrono::seconds>(std::chrono::system_clock::now().time_since_epoch()).count() : 0;
     cudaStream_t s = c->stream;
     // the window: a snapshot of the ring's head under the bookkeeping lock. Only drain-side calls (all under out_mu)
     // move the head or free segments, so the snapshot stays valid while the launch is prepared without c->mu.
@@ -1203,7 +1218,7 @@ static int64_t drain_launch_common(b9_ctx* c, int handler, uint32_t max_tasks, i
             if (a < b) { pieces.push_back(Piece{sg, a, b, !sg.drain_waited}); sg.drain_waited = true; win_pickle |= sg.n_pickle != 0; }
         }
     }
-    if (n == 0) { c->have_results = true; return 0; }
+    if (n == 0) { c->res.have = true; return 0; }
     uint64_t in_bytes = 0;                                                  // payload bytes of the window
     uint32_t win_max_len = 0; bool max_known = true;                        // its longest task, when every batch in it told
     for (const Piece& pc : pieces) { if (pc.sg.max_len) win_max_len = std::max(win_max_len, pc.sg.max_len); else max_known = false; }
@@ -1221,12 +1236,12 @@ static int64_t drain_launch_common(b9_ctx* c, int handler, uint32_t max_tasks, i
     DrainArgs a{};
     a.payload = c->d_payload; a.off = c->d_off; a.hdr = c->d_hdr; a.ids = c->d_ids; a.slot_mask = c->slot_mask;
     a.first_task = head; a.n_tasks = n; a.n_tiles = 0;                     // (set per handler by launch_drain3)
-    a.tile_base = (const uint32_t*)c->d_tile_state; a.block_base = (const uint32_t*)c->d_tile_state + ((size_t)c->max_drain_tasks / D2_THREADS + 2);
+    a.tile_base = (const uint32_t*)c->d_tile_state.v; a.block_base = (const uint32_t*)c->d_tile_state.v + ((size_t)c->max_drain_tasks / D2_THREADS + 2);
     a.count_mode = count_mode;
     a.slow = c->d_slow; a.crc_shift_tabs = c->d_crc_shift;
     a.static_rounds = 0;
     a.retry_mask = endpoint ? 0u : c->retry_mask; a.max_retries = c->max_retries; a.task_of = c->d_task_of;
-    c->res_retry = a.retry_mask != 0;
+    c->res.retry = a.retry_mask != 0;
     c->drain_epoch = (c->drain_epoch + 1u) & 0xFFFFFFu;
     if (c->drain_epoch == 0u) {                                             // the 24-bit tag wrapped: forget old tags
         c->drain_epoch = 1u; c->ctl_dirty = true;                           // (and the control ring's order)
@@ -1287,24 +1302,24 @@ static int64_t drain_launch_common(b9_ctx* c, int handler, uint32_t max_tasks, i
     // writer (drain3_kernel or the pickle pass). Like the pickle pass it is never a programmatic dependent, the next drain
     // kernel waits for it in full, and the timed span ends behind it. It reads this launch's control block and count
     // prefixes, which nothing rewrites before the next launch.
-    if (c->res_cb) {
+    if (c->res.cb) {
         a.tile_tasks = tt;
-        le = launch_callback_sign(&a, sizeof a, c->cb_mid, c->res_cb_keyed ? 1 : 0, c->res_cb_ts, c->d_cb_kind, c->d_cb_digest, c->sm_count, s);
+        le = launch_callback_sign(&a, sizeof a, c->cb_mid, c->res.cb_keyed ? 1 : 0, c->res.cb_ts, c->d_cb_kind, c->d_cb_digest, c->sm_count, s);
         if (le != cudaSuccess) { c->last_op_drain = false; c->ctl_dirty = true; return fail(B9_EIO, "callback sign pass launch failed: %s", cudaGetErrorString(le)); }
     }
-    if (pickle_pass || c->res_cb) end_drain_span(c);
+    if (pickle_pass || c->res.cb) end_drain_span(c);
     {
         std::lock_guard<std::mutex> lk(c->mu);
-        c->stats.kernel_launches += (a.count_mode ? 3 : 1) + (pickle_pass ? 1 : 0) + (c->res_cb ? 1 : 0);   // (+ tile_count_kernel and tile_scan_kernel)
+        c->stats.kernel_launches += (a.count_mode ? 3 : 1) + (pickle_pass ? 1 : 0) + (c->res.cb ? 1 : 0);   // (+ tile_count_kernel and tile_scan_kernel)
         c->stats.last_drain_tiles = (n + 127) / 128;                       // (reported in units of 128 tasks)
         c->stats.drains++;
     }
-    c->res_async = true; c->res_async_n = n; c->res_async_in_bytes = in_bytes;
-    c->res_ids_in_ring = !a.out.ids_compacted; c->res_head = head;        // (a burst of async launches: the last one's records wait)
-    if (!c->res_peek) c->running.store(n, std::memory_order_relaxed);
+    c->res.async = true; c->res.async_n = n; c->res.async_in_bytes = in_bytes;
+    c->res.ids_in_ring = !a.out.ids_compacted; c->res.head = head;        // (a burst of async launches: the last one's records wait)
+    if (!c->res.peek) c->running.store(n, std::memory_order_relaxed);
     if (peek & B9_DRAIN_ASYNC) return (int64_t)n;   // records = n minus the cancelled slots: known after b9_sync / b9_drain_fetch
     int rc = finish_launch(c);
-    return rc ? rc : (int64_t)c->res_n;
+    return rc ? rc : (int64_t)c->res.n;
 }
 
 int64_t b9_drain_launch(b9_ctx* c, int handler, uint32_t max_tasks, int peek) {
@@ -1327,37 +1342,33 @@ static int64_t drain_fetch(b9_ctx* c, b9_results* out, b9_callbacks* cb) {
     end_drain_span(c);
     CU(cudaSetDevice(c->device));
     { int rc = finish_launch(c); if (rc) return rc; }
-    if (!c->have_results) return fail(B9_EINVAL, "b9_drain_fetch: no drain results are waiting");
-    if (cb && !c->res_cb) return fail(B9_EINVAL, "b9_drain_fetch_callbacks: the waiting results come from a launch without a callback pass");
-    out->n_results = c->res_n; out->n_popped = c->res_popped; out->n_bytes = c->res_bytes; out->need_bytes = c->res_bytes;
+    if (!c->res.have) return fail(B9_EINVAL, "b9_drain_fetch: no drain results are waiting");
+    if (cb && !c->res.cb) return fail(B9_EINVAL, "b9_drain_fetch_callbacks: the waiting results come from a launch without a callback pass");
+    out->n_results = c->res.n; out->n_popped = c->res.popped; out->n_bytes = c->res.bytes; out->need_bytes = c->res.bytes;
     out->task_duration = 0.f;
-    if (cb) cb->timestamp = c->res_cb_ts;
-    if (c->res_n > out->cap_tasks || c->res_bytes > out->cap_bytes || (cb && c->res_n > cb->cap_tasks))
-        return fail(B9_ENOSPC, "b9_drain_fetch: need %u records / %llu bytes, caller gave %u / %llu (callbacks: %u)", c->res_n,
-                    (unsigned long long)c->res_bytes, out->cap_tasks, (unsigned long long)out->cap_bytes, cb ? cb->cap_tasks : 0u);
+    if (cb) cb->timestamp = c->res.cb_ts;
+    if (c->res.n > out->cap_tasks || c->res.bytes > out->cap_bytes || (cb && c->res.n > cb->cap_tasks))
+        return fail(B9_ENOSPC, "b9_drain_fetch: need %u records / %llu bytes, caller gave %u / %llu (callbacks: %u)", c->res.n,
+                    (unsigned long long)c->res.bytes, out->cap_tasks, (unsigned long long)out->cap_bytes, cb ? cb->cap_tasks : 0u);
     cudaStream_t s = c->stream;
-    const size_t n = c->res_n;
+    const size_t n = c->res.n;
     CU(cudaEventRecord(c->ev_c, s));
     if (n) {
         if (!out->task_ids || !out->status || !out->has_result || !out->offsets || !out->lengths) return fail(B9_EINVAL, "b9_drain_fetch: NULL result array");
         CU(cudaMemcpyAsync(out->lengths, c->d_out_len, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
-        if (c->res_ids_in_ring) {                                          // the window's slots: one piece, or two when it wraps the ring
-            const uint32_t slot0 = (uint32_t)(c->res_head & c->slot_mask);
-            const size_t first = std::min<size_t>(n, (size_t)c->slot_mask + 1u - slot0);
-            CU(cudaMemcpyAsync(out->task_ids, c->d_ids + slot0, first * 16, cudaMemcpyDeviceToHost, s));
-            if (first < n) CU(cudaMemcpyAsync(out->task_ids + first * 16, c->d_ids, (n - first) * 16, cudaMemcpyDeviceToHost, s));
-        } else CU(cudaMemcpyAsync(out->task_ids, c->d_out_ids, n * 16, cudaMemcpyDeviceToHost, s));
+        if (c->res.ids_in_ring) CU(copy_slot_ids(c, c->res.head, n, out->task_ids, false, cudaMemcpyDeviceToHost, s));   // (the window's slots)
+        else CU(cudaMemcpyAsync(out->task_ids, c->d_out_ids, n * 16, cudaMemcpyDeviceToHost, s));
         CU(cudaMemcpyAsync(out->status, c->d_out_status, n, cudaMemcpyDeviceToHost, s));
         CU(cudaMemcpyAsync(out->has_result, c->d_out_has, n, cudaMemcpyDeviceToHost, s));
         CU(cudaMemcpyAsync(out->offsets, c->d_out_off, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
-        if (c->res_bytes) {
+        if (c->res.bytes) {
             if (!out->payload) return fail(B9_EINVAL, "b9_drain_fetch: NULL payload buffer");
-            CU(cudaMemcpyAsync(out->payload, c->d_out_payload, c->res_bytes, cudaMemcpyDeviceToHost, s));
+            CU(cudaMemcpyAsync(out->payload, c->d_out_payload, c->res.bytes, cudaMemcpyDeviceToHost, s));
         }
         if (cb) {
             if (!cb->kind || !cb->digest) return fail(B9_EINVAL, "b9_drain_fetch_callbacks: NULL callback array");
             CU(cudaMemcpyAsync(cb->kind, c->d_cb_kind, n, cudaMemcpyDeviceToHost, s));
-            if (c->res_cb_keyed) CU(cudaMemcpyAsync(cb->digest, c->d_cb_digest, n * 32, cudaMemcpyDeviceToHost, s));
+            if (c->res.cb_keyed) CU(cudaMemcpyAsync(cb->digest, c->d_cb_digest, n * 32, cudaMemcpyDeviceToHost, s));
             else memset(cb->digest, 0, n * 32);                          // (without a key no digest is written)
         }
     }
@@ -1366,13 +1377,13 @@ static int64_t drain_fetch(b9_ctx* c, b9_results* out, b9_callbacks* cb) {
     float ms = 0; cudaEventElapsedTime(&ms, c->ev_c, c->ev_d);
     // the window's RETRY records (only a drain under a retry policy writes them), in record order: pushed again below
     std::vector<uint32_t> retry_rec;
-    if (!c->res_peek && c->res_retry)
+    if (!c->res.peek && c->res.retry)
         for (size_t j = 0; j < n; ++j) if (out->status[j] == B9_ST_RETRY) retry_rec.push_back((uint32_t)j);
     // TaskQueueCompleteRequest.task_duration (taskqueue.proto:50): the runner reports the seconds it spent on a task; a
-    // drain spends kernel + read-back time on res_popped tasks at once, so every task of the batch is charged its share
-    if (c->res_popped) out->task_duration = (c->res_kernel_ms + ms) * 1e-3f / (float)c->res_popped;
+    // drain spends kernel + read-back time on res.popped tasks at once, so every task of the batch is charged its share
+    if (c->res.popped) out->task_duration = (c->res.kernel_ms + ms) * 1e-3f / (float)c->res.popped;
     // the records, and with cb the kinds and (under a key) the digests
-    const uint64_t d2h_bytes = c->res_bytes + n * (16 + 1 + 1 + 8 + 4) + (cb ? n * (1 + (c->res_cb_keyed ? 32 : 0)) : 0);
+    const uint64_t d2h_bytes = c->res.bytes + n * (16 + 1 + 1 + 8 + 4) + (cb ? n * (1 + (c->res.cb_keyed ? 32 : 0)) : 0);
     if (!retry_rec.empty()) {
         // the re-push is a push: it takes the producers' lock, so that concurrent pushes land wholly before or after it. The
         // lock order is in_mu before out_mu: when a producer holds in_mu, out_mu is let go while the fetch waits for it, and
@@ -1383,7 +1394,7 @@ static int64_t drain_fetch(b9_ctx* c, b9_results* out, b9_callbacks* cb) {
             in_lk.lock();
             out_lk.lock();
             end_drain_span(c);
-            if (c->res_gen != gen || !c->have_results)
+            if (c->res_gen != gen || !c->res.have)
                 return fail(B9_EINVAL, "b9_drain_fetch: another drain-side call replaced or committed these results meanwhile");
         }
         const int rc = commit_with_repush(c, retry_rec, ms, d2h_bytes);
@@ -1392,11 +1403,12 @@ static int64_t drain_fetch(b9_ctx* c, b9_results* out, b9_callbacks* cb) {
         std::lock_guard<std::mutex> lk(c->mu);
         c->stats.last_drain_d2h_ms = ms;
         c->stats.bytes_d2h += d2h_bytes;
-        if (!c->res_peek) commit_pop(c);
+        if (!c->res.peek) commit_pop(c);
     }
-    if (!c->res_peek && c->recount_cancelled) { int rc = recount_cancelled_locked_out(c); if (rc) return rc; }
+    if (!c->res.peek && c->recount_cancelled) { int rc = recount_cancelled_locked_out(c); if (rc) return rc; }
+    c->res = WaitingResults{};
     c->running.store(0, std::memory_order_relaxed);
-    c->have_results = false; c->res_async = false; c->burst_open = false; c->res_gen++;
+    c->burst_open = false; c->res_gen++;
     return (int64_t)n;
 }
 
@@ -1451,8 +1463,10 @@ static int64_t wire_encode(b9_ctx* c, const b9_wire_env* env, uint32_t max_tasks
     if (!c || !env || !env->workspace_name || !env->stub_id) return fail(B9_EINVAL, "%s: NULL argument", fn);
     OutLock out_lk(c);
     CU(cudaSetDevice(c->device));
-    c->have_results = false; c->res_async = false; c->burst_open = false;
+    c->res = WaitingResults{};
     c->running.store(0, std::memory_order_relaxed);
+    c->burst_open = false; c->res_gen++;
+    c->res.peek = true;
     uint64_t head = 0; uint32_t n = 0;
     cudaStream_t s = c->stream;
     {
@@ -1460,11 +1474,9 @@ static int64_t wire_encode(b9_ctx* c, const b9_wire_env* env, uint32_t max_tasks
         head = c->head_task;
         const uint64_t depth = c->tail_task - c->head_task;
         n = (uint32_t)std::min<uint64_t>(std::min<uint64_t>(depth, max_tasks), c->max_drain_tasks);
-        for (const Segment& sg : c->segs) CU(cudaStreamWaitEvent(s, sg.ready, 0));
+        if (const int rc = wait_pending(c, s)) return rc;
     }
-    c->res_n = 0; c->res_popped = 0; c->res_bytes = 0; c->res_in_bytes = 0; c->res_peek = true;
-    c->res_gen++; c->res_retry = false; c->res_cb = false;
-    if (n == 0) { c->have_results = true; return 0; }
+    if (n == 0) { c->res.have = true; return 0; }
     WireEnv we; memset(&we, 0, sizeof we);
     {
         uint8_t* o = we.mid; size_t k = 0; const size_t cap = sizeof we.mid;
@@ -1484,7 +1496,7 @@ static int64_t wire_encode(b9_ctx* c, const b9_wire_env* env, uint32_t max_tasks
     a.payload = c->d_payload; a.off = c->d_off; a.hdr = c->d_hdr; a.ids = c->d_ids; a.ts = c->d_ts; a.exp = c->d_exp;
     a.slot_mask = c->slot_mask; a.first_task = head; a.n_tasks = n;
     a.out = drain_out(c, c->d_ctl, false);                                  // (a record for every task of the window)
-    c->res_ids_in_ring = !a.out.ids_compacted; c->res_head = head;
+    c->res.ids_in_ring = !a.out.ids_compacted; c->res.head = head;
     CU(cudaEventRecord(c->ev_a, s));
     if (full) CU(launch_wire_encode_full(&a, sizeof a, c->d_wire_env, (n + 127) / 128, s));
     else wire_encode_kernel<false><<<(n + 127) / 128, 128, 0, s>>>(a, c->d_wire_env);
@@ -1493,11 +1505,11 @@ static int64_t wire_encode(b9_ctx* c, const b9_wire_env* env, uint32_t max_tasks
     CU(cudaMemcpyAsync(c->h_ctl, c->d_ctl, sizeof(DrainCtl), cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));     // (the stack copy of `we` is consumed by now as well)
     if (c->h_ctl->overflow) return fail(B9_ENOSPC, "%s: records exceed max_result_bytes (%llu)", fn, (unsigned long long)c->max_result_bytes);
-    c->res_bytes = c->h_ctl->bytes; c->res_n = n; c->res_popped = 0; c->have_results = true;
-    float ms = 0; cudaEventElapsedTime(&ms, c->ev_a, c->ev_b); c->res_kernel_ms = ms;
+    c->res.bytes = c->h_ctl->bytes; c->res.n = n; c->res.popped = 0; c->res.have = true;
+    float ms = 0; cudaEventElapsedTime(&ms, c->ev_a, c->ev_b); c->res.kernel_ms = ms;
     std::lock_guard<std::mutex> lk(c->mu);
     c->stats.kernel_launches++;
-    c->stats.last_drain_out_bytes = c->res_bytes;
+    c->stats.last_drain_out_bytes = c->res.bytes;
     c->stats.last_drain_kernel_ms = ms;
     return (int64_t)n;
 }
@@ -1685,13 +1697,14 @@ MetaLayout meta_layout(uint64_t n) {
     m.total = o; return m;
 }
 
-// drop k tasks from the tail of the ring (they were handed to another rank); cut_phys = physical offset of the first dropped task
+// drop k tasks from the tail of the ring (they were handed to another rank); cut_phys = physical offset of the first dropped
+// task. Caller holds c->mu.
 void drop_back(b9_ctx* c, uint64_t k, uint64_t cut_phys) {
     while (k && !c->segs.empty()) {
         Segment& sg = c->segs.back();
         if (sg.n <= k) {
             k -= sg.n; c->tail_task -= sg.n; c->pending_bytes -= sg.bytes; c->write_pos = sg.phys_start;
-            c->event_pool.push_back(sg.ready); c->segs.pop_back();
+            put_event(c, sg.ready); c->segs.pop_back();
         } else {
             const uint32_t keep = sg.n - (uint32_t)k;
             const uint64_t nb = cut_phys - sg.phys_start;               // (the cut lies inside this segment)
@@ -1740,20 +1753,19 @@ int b9_comm_init(b9_ctx* c, const uint8_t* id128, int rank, int world) {
         // everything the planning phase of b9_rebalance touches is allocated here, once: the byte prefix of a full slot ring,
         // the block sums of its scan, the all-gather tables and the page-locked block the cut points come back in
         if (!c->d_prefix) {
-            CU(cudaMalloc(&c->d_prefix, ((size_t)c->ring_tasks + 2) * sizeof(uint64_t)));
-            CU(cudaMalloc(&c->d_scan_sums, ((size_t)c->ring_tasks / SCAN_BLOCK + 2) * sizeof(unsigned long long)));
+            CU(cudaMalloc(&c->d_prefix.v, ((size_t)c->ring_tasks + 2) * sizeof(uint64_t)));
+            CU(cudaMalloc(&c->d_scan_sums.v, ((size_t)c->ring_tasks / SCAN_BLOCK + 2) * sizeof(unsigned long long)));
         }
         if (!c->d_rtab) {
             c->rtab_words = 4 * (size_t)REBALANCE_MAX_WORLD * 2 + 2 * (size_t)REBALANCE_MAX_WORLD * (REBALANCE_MAX_WORLD + 1) + (size_t)REBALANCE_MAX_WORLD + sizeof(RebalanceCuts) / 8 + 16;
-            CU(cudaMalloc(&c->d_rtab, c->rtab_words * sizeof(uint64_t)));
-            CU(cudaHostAlloc(&c->h_rtab, c->rtab_words * sizeof(uint64_t), cudaHostAllocDefault));
+            CU(cudaMalloc(&c->d_rtab.v, c->rtab_words * sizeof(uint64_t)));
+            CU(cudaHostAlloc(&c->h_rtab.v, c->rtab_words * sizeof(uint64_t), cudaHostAllocDefault));
         }
-        // ... and a first size for the two arenas the slot words (and non-contiguous payload ranges) are staged in
+        // ... and a first size for the two arenas the slot words (and non-contiguous payload ranges) are staged in (a failure
+        // here is not an error: b9_rebalance grows them to what it needs)
         const uint64_t first = std::max<uint64_t>((uint64_t)c->ring_tasks * 48 / 2, 16ull << 20);
-        if (c->xchg_send_cap < first) { cudaFree(c->d_xchg_send); c->d_xchg_send = nullptr; c->xchg_send_cap = 0;
-                                        if (cudaMalloc(&c->d_xchg_send, first) == cudaSuccess) c->xchg_send_cap = first; else cudaGetLastError(); }
-        if (c->xchg_recv_cap < first) { cudaFree(c->d_xchg_recv); c->d_xchg_recv = nullptr; c->xchg_recv_cap = 0;
-                                        if (cudaMalloc(&c->d_xchg_recv, first) == cudaSuccess) c->xchg_recv_cap = first; else cudaGetLastError(); }
+        (void)c->d_xchg_send.grow(first);
+        (void)c->d_xchg_recv.grow(first);
     }
     // NCCL sets its point-to-point channels up lazily, on the first send/recv of every pair and of every
     // channel a message is spread over (seconds on an 8-GPU box): do that here, once, with an all-to-all
@@ -1762,8 +1774,8 @@ int b9_comm_init(b9_ctx* c, const uint8_t* id128, int rank, int world) {
     if (world > 1) {
         size_t per = 4u << 20;
         if (const char* e = getenv("B9_COMM_WARMUP_BYTES")) per = (size_t)std::max<long long>(16, atoll(e));
-        uint8_t* d = nullptr;
-        CU(cudaMalloc(&d, (size_t)world * per * 2));
+        DevPtr<uint8_t> d;
+        CU(cudaMalloc(&d.v, (size_t)world * per * 2));
         CU(cudaMemsetAsync(d, 0, (size_t)world * per * 2, c->stream));
         NC(g_nccl.AllGather(d, d + per, 16, NCCL_U64, comm, c->stream));      // (world * 128 bytes <= per)
         NC(g_nccl.GroupStart());
@@ -1774,7 +1786,6 @@ int b9_comm_init(b9_ctx* c, const uint8_t* id128, int rank, int world) {
         }
         NC(g_nccl.GroupEnd());
         CU(cudaStreamSynchronize(c->stream));
-        cudaFree(d);
     }
     return B9_OK;
 }
@@ -1815,9 +1826,10 @@ int b9_rebalance(b9_ctx* c, b9_rebalance_info* info) {
         if (info) { memset(info, 0, sizeof *info); info->world = 1; info->tasks_before = info->tasks_after = c->tail_task - c->head_task; info->bytes_before = info->bytes_after = c->pending_bytes; }
         return B9_OK;
     }
-    for (const Segment& sg : c->segs) CU(cudaStreamWaitEvent(s, sg.ready, 0));
-    c->have_results = false; c->res_async = false; c->burst_open = false;
+    if (const int rc = wait_pending(c, s)) return rc;
+    c->res = WaitingResults{};
     c->running.store(0, std::memory_order_relaxed);
+    c->burst_open = false;
     free_segments(c);
     const uint64_t n = c->tail_task - c->head_task;
     const uint64_t my_bytes = c->pending_bytes;
@@ -1900,17 +1912,8 @@ int b9_rebalance(b9_ctx* c, b9_rebalance_info* info) {
         const uint64_t rk = M_tasks(d, R);
         if (rk) need_r += al(meta_layout(rk).total);
     }
-    auto ensure = [&](uint8_t*& buf, uint64_t& cap, uint64_t need) -> cudaError_t {
-        if (need <= cap) return cudaSuccess;
-        if (buf) cudaFree(buf);
-        buf = nullptr; cap = 0;
-        const uint64_t want = need + need / 4;
-        cudaError_t e = cudaMalloc(&buf, want);
-        if (e == cudaSuccess) cap = want;
-        return e;
-    };
-    CU(ensure(c->d_xchg_send, c->xchg_send_cap, need_s));
-    CU(ensure(c->d_xchg_recv, c->xchg_recv_cap, need_r));
+    { const int rc = c->d_xchg_send.ensure(need_s, "b9_rebalance: send staging", need_s / 4); if (rc) return rc; }
+    { const int rc = c->d_xchg_recv.ensure(need_r, "b9_rebalance: receive staging", need_r / 4); if (rc) return rc; }
     std::vector<uint8_t*> s_meta(W, nullptr), r_meta(W, nullptr);
     std::vector<const uint8_t*> s_pay(W, nullptr);
     uint64_t so = 0, ro = 0;
@@ -1966,33 +1969,24 @@ int b9_rebalance(b9_ctx* c, b9_rebalance_info* info) {
         const MetaLayout ml = meta_layout(rk);
         const uint64_t pb = M_bytes(src, R);
         const uint64_t start = r_start[src];
-        // slot words: ids may wrap in the slot ring
-        const uint32_t slot0 = (uint32_t)(c->tail_task & c->slot_mask);
-        const uint32_t first = (uint32_t)std::min<uint64_t>(rk, c->ring_tasks - slot0);
-        CU(cudaMemcpyAsync(c->d_ids + slot0, r_meta[src] + ml.ids, (size_t)first * 16, cudaMemcpyDeviceToDevice, s));
-        if (first < rk) CU(cudaMemcpyAsync(c->d_ids, r_meta[src] + ml.ids + (size_t)first * 16, (size_t)(rk - first) * 16, cudaMemcpyDeviceToDevice, s));
+        CU(copy_slot_ids(c, c->tail_task, rk, r_meta[src] + ml.ids, true, cudaMemcpyDeviceToDevice, s));
         ingest_kernel<<<(uint32_t)((rk + 255) / 256), 256, 0, s>>>((const uint64_t*)(r_meta[src] + ml.rel), (uint32_t)rk, start, c->tail_task, c->slot_mask,
                                                                   (const int64_t*)(r_meta[src] + ml.ts), (const int64_t*)(r_meta[src] + ml.exp),
                                                                   r_meta[src] + ml.retries, r_meta[src] + ml.flags, c->d_off, c->d_hdr, c->d_ts, c->d_exp);
         CU(cudaGetLastError());
         c->stats.kernel_launches++;
         cudaEvent_t ready;
-        if (!c->event_pool.empty()) { ready = c->event_pool.back(); c->event_pool.pop_back(); }
-        else CU(cudaEventCreateWithFlags(&ready, cudaEventDisableTiming));
+        CU(take_event(c, &ready));
         CU(cudaEventRecord(ready, s));
-        c->segs.push_back(Segment{c->tail_task, (uint32_t)rk, start, pb, ready, 0u});
-        c->segs.back().n_pickle = (uint32_t)rk;
-        c->write_pos = start + b9_seg_span(pb);
-        c->tail_task += rk; c->pending_bytes += pb;
+        append_segment(c, (uint32_t)rk, start, pb, 0u, (uint32_t)rk, ready);   // (max_len and the pickle tasks not known)
     }
     // ---- cancelled tasks may have moved either way: recount over the new window (only if some rank held any)
     if (any_cancelled) {
         const uint64_t depth = c->tail_task - c->head_task;
-        CU(cudaMemsetAsync(c->d_count, 0, sizeof(unsigned long long), s));
-        if (depth) { count_cancelled_kernel<<<(uint32_t)((depth + 255) / 256), 256, 0, s>>>(c->d_hdr, c->slot_mask, c->head_task, (uint32_t)depth, c->d_count); CU(cudaGetLastError()); c->stats.kernel_launches++; }
-        CU(cudaMemcpyAsync(c->h_count, c->d_count, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
-        CU(cudaStreamSynchronize(s));
-        c->cancelled_pending = *c->h_count;
+        uint64_t count = 0;
+        { const int rc = count_cancelled(c, c->head_task, depth, s, &count); if (rc) return rc; }
+        if (depth) c->stats.kernel_launches++;
+        c->cancelled_pending = count;
     } else {
         CU(cudaStreamSynchronize(s));         // the caller's next call may be on any stream; the exchange is complete when we return
         c->cancelled_pending = 0;
@@ -2034,8 +2028,8 @@ int64_t b9_drain_fetch_object(b9_ctx* c, uint8_t* obj, uint64_t cap, uint64_t* o
         OutLock out_lk(c);
         CU(cudaSetDevice(c->device));
         { int rc = finish_launch(c); if (rc) return rc; }
-        if (!c->have_results) return fail(B9_EINVAL, "b9_drain_fetch_object: no drain results are waiting");
-        n = c->res_n; bytes = c->res_bytes;
+        if (!c->res.have) return fail(B9_EINVAL, "b9_drain_fetch_object: no drain results are waiting");
+        n = c->res.n; bytes = c->res.bytes;
     }
     const b9sink::Layout L = b9sink::layout(n, bytes);
     if (object_bytes) *object_bytes = L.total;
