@@ -18,6 +18,7 @@ TF_HTTP_BODY, TF_PICKLE, TF_TASK_MSG = 0x02, 0x04, 0x08
 CANCEL_MARKED, CANCEL_ALREADY, CANCEL_CLAIMED = 0x01, 0x02, 0x04      # b9_cancel outcome bits
 DRAIN_PEEK, DRAIN_ASYNC, DRAIN_PICKLE_FULL = 1, 2, 4                   # b9_drain_launch flags
 CB_NONE, CB_POST, CB_UNSENDABLE, CB_HOST = 0, 1, 2, 3                  # enum b9_callback_kind
+CB_RUNNER_FUNCTION, CB_RUNNER_ENDPOINT = 0x1, 0x2                       # b9_set_callback_runners bits
 
 
 class Opts(C.Structure):
@@ -40,6 +41,11 @@ class Results(C.Structure):
 
 class Callbacks(C.Structure):
     _fields_ = [("kind", C.c_void_p), ("digest", C.c_void_p), ("cap_tasks", C.c_uint32), ("timestamp", C.c_int64)]
+
+
+class CallbackRequests(C.Structure):
+    _fields_ = [("body_offsets", C.c_void_p), ("body_lengths", C.c_void_p), ("url_offsets", C.c_void_p),
+                ("url_lengths", C.c_void_p), ("cap_tasks", C.c_uint32)]
 
 
 class Stats(C.Structure):
@@ -91,6 +97,8 @@ SYMBOLS = {
     "b9_set_retry_policy": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32]),
     "b9_set_callback_policy": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_uint32]),
     "b9_drain_fetch_callbacks": (C.c_int64, [C.c_void_p, C.POINTER(Results), C.POINTER(Callbacks)]),
+    "b9_set_callback_runners": (C.c_int, [C.c_void_p, C.c_uint32]),
+    "b9_drain_fetch_callback_requests": (C.c_int64, [C.c_void_p, C.POINTER(Results), C.POINTER(Callbacks), C.POINTER(CallbackRequests)]),
     "b9_drain": (C.c_int64, [C.c_void_p, C.c_int, C.c_uint32, C.POINTER(Results)]),
     "b9_drain_launch": (C.c_int64, [C.c_void_p, C.c_int, C.c_uint32, C.c_int]),
     "b9_drain_fetch": (C.c_int64, [C.c_void_p, C.POINTER(Results)]),

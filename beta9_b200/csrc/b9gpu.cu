@@ -52,6 +52,10 @@ cudaError_t launch_callback_sign(const void* args, size_t args_size, const uint3
 // = ENDPOINT_TILE_TASKS and n_tiles set for it
 cudaError_t launch_endpoint_drain(const void* args, size_t args_size, int handler, int sm_count, cudaStream_t s);
 constexpr uint32_t ENDPOINT_TILE_TASKS = 32;   // endpoint_drain.cu's EP_TILE (the launcher refuses any other)
+// the function runner's callback pass (in place of the pickle pass, behind callback_sign_kernel) or the endpoint runner's
+// (behind endpoint_drain_kernel), from callback_runners.cu; out: kind, digest, body_off, body_len, url_off, url_len
+cudaError_t launch_callback_runner(int endpoint, const void* args, size_t args_size, int handler, const uint32_t mid[16], int keyed,
+                                   int64_t ts, void* const out[6], int sm_count, cudaStream_t s);
 
 using namespace b9;
 
@@ -165,6 +169,7 @@ struct WaitingResults {
     bool have = false, peek = false;
     bool retry = false;                        // they come from a drain launched under a retry policy
     bool cb = false, cb_keyed = false; int64_t cb_ts = 0;   // ... with a callback pass: its keying and Unix seconds
+    bool cb_requests = false;                  // ... and a runner's callback pass wrote the request arrays (else they are R)
     uint32_t n = 0, popped = 0; uint64_t bytes = 0, in_bytes = 0; float kernel_ms = 0.f;
     bool ids_in_ring = false; uint64_t head = 0;   // record j's id is the ring id of task head + j (DrainOut::ids_compacted == 0)
     bool async = false;                        // the last launch returned before its kernels finished: finalize on fetch / sync
@@ -213,6 +218,11 @@ struct b9_ctx {
     bool cb_enabled = false, cb_keyed = false; uint32_t cb_mid[16] = {};
     GrowBuf<uint8_t> d_cb_kind;                // [max_drain_tasks] b9_callback_kind per record
     GrowBuf<uint8_t> d_cb_digest;              // [max_drain_tasks * 32] raw HMAC-SHA256 per record
+    // the runners whose callbacks are settled on the device too (b9_set_callback_runners; set under out_mu) and their
+    // passes' request arrays (allocated with the first runner): D and the task's own URL per record, in d_out_payload
+    uint32_t cb_runners = 0;
+    GrowBuf<uint64_t> d_cb_body_off, d_cb_url_off;   // [max_drain_tasks]
+    GrowBuf<uint32_t> d_cb_body_len, d_cb_url_len;   // [max_drain_tasks]
     // ring bookkeeping (host)
     uint64_t head_task = 0, tail_task = 0;     // logical, monotonically increasing
     uint64_t write_pos = 0;                    // physical byte position of the next segment
@@ -708,6 +718,23 @@ int b9_set_callback_policy(b9_ctx* c, int enabled, const uint8_t* signing_key, u
     return B9_OK;
 }
 
+int b9_set_callback_runners(b9_ctx* c, uint32_t runners) {
+    if (!c) return fail(B9_EINVAL, "b9_set_callback_runners: ctx is NULL");
+    if (runners & ~(uint32_t)(B9_CB_RUNNER_FUNCTION | B9_CB_RUNNER_ENDPOINT)) return fail(B9_EINVAL, "b9_set_callback_runners: unknown bits 0x%x", runners);
+    OutLock out_lk(c);
+    if (runners) {
+        CU(cudaSetDevice(c->device));
+        const uint64_t md = c->max_drain_tasks;
+        int rc = c->d_cb_body_off.ensure(md * sizeof(uint64_t), "b9_set_callback_runners: body offsets");   // (ensure takes bytes)
+        if (rc == B9_OK) rc = c->d_cb_body_len.ensure(md * sizeof(uint32_t), "b9_set_callback_runners: body lengths");
+        if (rc == B9_OK) rc = c->d_cb_url_off.ensure(md * sizeof(uint64_t), "b9_set_callback_runners: URL offsets");
+        if (rc == B9_OK) rc = c->d_cb_url_len.ensure(md * sizeof(uint32_t), "b9_set_callback_runners: URL lengths");
+        if (rc) return rc;
+    }
+    c->cb_runners = runners;
+    return B9_OK;
+}
+
 int b9_device_count(void) {
     int n = 0;
     if (cudaGetDeviceCount(&n) != cudaSuccess) { cudaGetLastError(); return 0; }
@@ -1196,7 +1223,7 @@ static int64_t drain_launch_common(b9_ctx* c, int handler, uint32_t max_tasks, i
     c->res_gen++;
     c->res.peek = (peek & B9_DRAIN_PEEK) != 0;
     // the callback pass signs with the host clock's Unix seconds, read once per launch (SignPayload's time.Now().Unix())
-    c->res.cb = !endpoint && c->cb_enabled; c->res.cb_keyed = c->res.cb && c->cb_keyed;
+    c->res.cb = c->cb_enabled && (!endpoint || (c->cb_runners & B9_CB_RUNNER_ENDPOINT)); c->res.cb_keyed = c->res.cb && c->cb_keyed;
     c->res.cb_ts = c->res.cb_keyed ? (int64_t)std::chrono::duration_cast<std::chrono::seconds>(std::chrono::system_clock::now().time_since_epoch()).count() : 0;
     cudaStream_t s = c->stream;
     // the window: a snapshot of the ring's head under the bookkeeping lock. Only drain-side calls (all under out_mu)
@@ -1277,7 +1304,7 @@ static int64_t drain_launch_common(b9_ctx* c, int handler, uint32_t max_tasks, i
         if (le != cudaSuccess) { c->ctl_dirty = true; return fail(B9_EIO, "endpoint drain kernel launch failed: %s", cudaGetErrorString(le)); }
         c->last_op_drain = true;
         c->burst_open = true;
-        end_drain_span(c);
+        if (!c->res.cb) end_drain_span(c);                                  // (with the runner's callback pass: behind that)
     } else switch (handler) {
     case B9_H_IDENTITY: le = launch_drain3<0>(a, in_bytes / n, win_max_len, c->stage_bytes_override, c->sm_count, overlap, s, &grid, &tt); break;
     case B9_H_CRC32:    le = launch_drain3<1>(a, in_bytes / n, win_max_len, c->stage_bytes_override, c->sm_count, overlap, s, &grid, &tt); break;
@@ -1293,7 +1320,11 @@ static int64_t drain_launch_common(b9_ctx* c, int handler, uint32_t max_tasks, i
     // drain3_kernel left UNSUPPORTED. The next drain kernel waits for it in full (no programmatic dependent launch), and
     // the timed span ends behind it.
     const bool pickle_pass = !endpoint && (peek & B9_DRAIN_PICKLE_FULL) && win_pickle;
-    if (pickle_pass) {
+    // the function runner's callbacks (b9_set_callback_runners): its pass does the pickle pass's work and runs behind the
+    // sign pass, whose B9_CB_HOST it overwrites for the pickle slots
+    const bool function_runner = pickle_pass && c->res.cb && (c->cb_runners & B9_CB_RUNNER_FUNCTION);
+    void* const rq_out[6] = {c->d_cb_kind, c->d_cb_digest, c->d_cb_body_off, c->d_cb_body_len, c->d_cb_url_off, c->d_cb_url_len};
+    if (pickle_pass && !function_runner) {
         a.tile_tasks = tt;
         le = launch_pickle_pass(&a, sizeof a, handler, c->sm_count, s);
         if (le != cudaSuccess) { c->last_op_drain = false; c->ctl_dirty = true; return fail(B9_EIO, "pickle pass launch failed: %s", cudaGetErrorString(le)); }
@@ -1301,11 +1332,20 @@ static int64_t drain_launch_common(b9_ctx* c, int handler, uint32_t max_tasks, i
     // under a callback policy: every record's callback kind and signature (callback_sign.cu), behind the records' last
     // writer (drain3_kernel or the pickle pass). Like the pickle pass it is never a programmatic dependent, the next drain
     // kernel waits for it in full, and the timed span ends behind it. It reads this launch's control block and count
-    // prefixes, which nothing rewrites before the next launch.
-    if (c->res.cb) {
+    // prefixes, which nothing rewrites before the next launch. The runners' passes (callback_runners.cu) follow the same rules.
+    if (c->res.cb && endpoint) {
+        le = launch_callback_runner(1, &a, sizeof a, handler, c->cb_mid, c->res.cb_keyed ? 1 : 0, c->res.cb_ts, rq_out, c->sm_count, s);
+        if (le != cudaSuccess) { c->last_op_drain = false; c->ctl_dirty = true; return fail(B9_EIO, "endpoint callback pass launch failed: %s", cudaGetErrorString(le)); }
+        c->res.cb_requests = true;
+    } else if (c->res.cb) {
         a.tile_tasks = tt;
         le = launch_callback_sign(&a, sizeof a, c->cb_mid, c->res.cb_keyed ? 1 : 0, c->res.cb_ts, c->d_cb_kind, c->d_cb_digest, c->sm_count, s);
         if (le != cudaSuccess) { c->last_op_drain = false; c->ctl_dirty = true; return fail(B9_EIO, "callback sign pass launch failed: %s", cudaGetErrorString(le)); }
+        if (function_runner) {
+            le = launch_callback_runner(0, &a, sizeof a, handler, c->cb_mid, c->res.cb_keyed ? 1 : 0, c->res.cb_ts, rq_out, c->sm_count, s);
+            if (le != cudaSuccess) { c->last_op_drain = false; c->ctl_dirty = true; return fail(B9_EIO, "function callback pass launch failed: %s", cudaGetErrorString(le)); }
+            c->res.cb_requests = true;
+        }
     }
     if (pickle_pass || c->res.cb) end_drain_span(c);
     {
@@ -1335,8 +1375,9 @@ int64_t b9_endpoint_drain_launch(b9_ctx* c, int handler, uint32_t max_tasks, int
     return drain_launch_common(c, handler, max_tasks, flags, true);
 }
 
-// b9_drain_fetch, and with cb (b9_drain_fetch_callbacks) the launch's callback kinds and digests in the same read-back
-static int64_t drain_fetch(b9_ctx* c, b9_results* out, b9_callbacks* cb) {
+// b9_drain_fetch, and with cb (b9_drain_fetch_callbacks) the launch's callback kinds and digests in the same read-back;
+// with rq too (b9_drain_fetch_callback_requests) each record's D and URL
+static int64_t drain_fetch(b9_ctx* c, b9_results* out, b9_callbacks* cb, b9_callback_requests* rq = nullptr) {
     std::unique_lock<std::mutex> in_lk(c->in_mu, std::defer_lock);
     std::unique_lock<std::mutex> out_lk(c->out_mu);
     end_drain_span(c);
@@ -1344,12 +1385,17 @@ static int64_t drain_fetch(b9_ctx* c, b9_results* out, b9_callbacks* cb) {
     { int rc = finish_launch(c); if (rc) return rc; }
     if (!c->res.have) return fail(B9_EINVAL, "b9_drain_fetch: no drain results are waiting");
     if (cb && !c->res.cb) return fail(B9_EINVAL, "b9_drain_fetch_callbacks: the waiting results come from a launch without a callback pass");
+    // a runner's pass signed each callback's D, which is not the record: only the fetch that returns D may hand them out
+    if (cb && !rq && c->res.cb_requests)
+        return fail(B9_EINVAL, "b9_drain_fetch_callbacks: the waiting results come from a launch with a runner's callback pass; "
+                               "their signed bodies come with b9_drain_fetch_callback_requests");
     out->n_results = c->res.n; out->n_popped = c->res.popped; out->n_bytes = c->res.bytes; out->need_bytes = c->res.bytes;
     out->task_duration = 0.f;
     if (cb) cb->timestamp = c->res.cb_ts;
-    if (c->res.n > out->cap_tasks || c->res.bytes > out->cap_bytes || (cb && c->res.n > cb->cap_tasks))
-        return fail(B9_ENOSPC, "b9_drain_fetch: need %u records / %llu bytes, caller gave %u / %llu (callbacks: %u)", c->res.n,
-                    (unsigned long long)c->res.bytes, out->cap_tasks, (unsigned long long)out->cap_bytes, cb ? cb->cap_tasks : 0u);
+    if (c->res.n > out->cap_tasks || c->res.bytes > out->cap_bytes || (cb && c->res.n > cb->cap_tasks) || (rq && c->res.n > rq->cap_tasks))
+        return fail(B9_ENOSPC, "b9_drain_fetch: need %u records / %llu bytes, caller gave %u / %llu (callbacks: %u, requests: %u)", c->res.n,
+                    (unsigned long long)c->res.bytes, out->cap_tasks, (unsigned long long)out->cap_bytes, cb ? cb->cap_tasks : 0u,
+                    rq ? rq->cap_tasks : 0u);
     cudaStream_t s = c->stream;
     const size_t n = c->res.n;
     CU(cudaEventRecord(c->ev_c, s));
@@ -1371,9 +1417,24 @@ static int64_t drain_fetch(b9_ctx* c, b9_results* out, b9_callbacks* cb) {
             if (c->res.cb_keyed) CU(cudaMemcpyAsync(cb->digest, c->d_cb_digest, n * 32, cudaMemcpyDeviceToHost, s));
             else memset(cb->digest, 0, n * 32);                          // (without a key no digest is written)
         }
+        if (rq) {
+            if (!rq->body_offsets || !rq->body_lengths || !rq->url_offsets || !rq->url_lengths) return fail(B9_EINVAL, "b9_drain_fetch_callback_requests: NULL request array");
+            if (c->res.cb_requests) {
+                CU(cudaMemcpyAsync(rq->body_offsets, c->d_cb_body_off, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
+                CU(cudaMemcpyAsync(rq->body_lengths, c->d_cb_body_len, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+                CU(cudaMemcpyAsync(rq->url_offsets, c->d_cb_url_off, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
+                CU(cudaMemcpyAsync(rq->url_lengths, c->d_cb_url_len, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+            }
+        }
     }
     CU(cudaEventRecord(c->ev_d, s));
     CU(cudaStreamSynchronize(s));
+    // a launch without a runner's pass (task-queue records only): every record's D is its own R, or {} without result bytes
+    if (rq && n && !c->res.cb_requests)
+        for (size_t j = 0; j < n; ++j) {
+            rq->body_offsets[j] = out->offsets[j]; rq->body_lengths[j] = out->has_result[j] ? out->lengths[j] : 0u;
+            rq->url_offsets[j] = 0; rq->url_lengths[j] = 0;
+        }
     float ms = 0; cudaEventElapsedTime(&ms, c->ev_c, c->ev_d);
     // the window's RETRY records (only a drain under a retry policy writes them), in record order: pushed again below
     std::vector<uint32_t> retry_rec;
@@ -1383,7 +1444,8 @@ static int64_t drain_fetch(b9_ctx* c, b9_results* out, b9_callbacks* cb) {
     // drain spends kernel + read-back time on res.popped tasks at once, so every task of the batch is charged its share
     if (c->res.popped) out->task_duration = (c->res.kernel_ms + ms) * 1e-3f / (float)c->res.popped;
     // the records, and with cb the kinds and (under a key) the digests
-    const uint64_t d2h_bytes = c->res.bytes + n * (16 + 1 + 1 + 8 + 4) + (cb ? n * (1 + (c->res.cb_keyed ? 32 : 0)) : 0);
+    const uint64_t d2h_bytes = c->res.bytes + n * (16 + 1 + 1 + 8 + 4) + (cb ? n * (1 + (c->res.cb_keyed ? 32 : 0)) : 0) +
+                               (rq && c->res.cb_requests ? n * (8 + 4 + 8 + 4) : 0);
     if (!retry_rec.empty()) {
         // the re-push is a push: it takes the producers' lock, so that concurrent pushes land wholly before or after it. The
         // lock order is in_mu before out_mu: when a producer holds in_mu, out_mu is let go while the fetch waits for it, and
@@ -1420,6 +1482,11 @@ int64_t b9_drain_fetch(b9_ctx* c, b9_results* out) {
 int64_t b9_drain_fetch_callbacks(b9_ctx* c, b9_results* out, b9_callbacks* cb) {
     if (!c || !out || !cb) return fail(B9_EINVAL, "b9_drain_fetch_callbacks: NULL argument");
     return drain_fetch(c, out, cb);
+}
+
+int64_t b9_drain_fetch_callback_requests(b9_ctx* c, b9_results* out, b9_callbacks* cb, b9_callback_requests* rq) {
+    if (!c || !out || !cb || !rq) return fail(B9_EINVAL, "b9_drain_fetch_callback_requests: NULL argument");
+    return drain_fetch(c, out, cb, rq);
 }
 
 int64_t b9_drain(b9_ctx* c, int handler, uint32_t max_tasks, b9_results* out) {

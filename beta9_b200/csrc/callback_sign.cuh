@@ -311,7 +311,7 @@ __device__ inline bool cb_kwargs_have_callback_url(const uint8_t* __restrict__ p
 
 }  // namespace b9
 
-#ifdef __CUDACC__
+#if defined(__CUDACC__) && !defined(B9_CALLBACK_NO_SIGN_KERNEL)   // (callback_runners.cu uses the signing code only)
 namespace b9 {
 // One pass over a drain's records, right after the drain kernel (and the pickle pass). Thread per window task: its record
 // index is the task's in a dense window, else the count pre-pass's tile prefix plus the tile's ready slots before it

@@ -51,6 +51,11 @@ class DrainResult:
     cb_kind: Optional[np.ndarray] = None     # uint8 [n]     CB_NONE / CB_POST / CB_UNSENDABLE / CB_HOST
     cb_digest: Optional[np.ndarray] = None   # uint8 [n,32]  raw HMAC-SHA256 of a CB_POST record under a key, else zero
     cb_timestamp: int = 0                    # the Unix seconds every digest signs (0: no key)
+    # under set_callback_runners (b9_drain_fetch_callback_requests): each record's callback JSON D and own URL in `payload`
+    cb_body_off: Optional[np.ndarray] = None  # uint64 [n]
+    cb_body_len: Optional[np.ndarray] = None  # uint32 [n]   0: D is {}
+    cb_url_off: Optional[np.ndarray] = None   # uint64 [n]
+    cb_url_len: Optional[np.ndarray] = None   # uint32 [n]   0: the stub's URL
 
     @property
     def n(self) -> int:
@@ -74,9 +79,21 @@ class DrainResult:
         return self.payload[src]
 
     def callback_body(self, i: int) -> bytes:
-        """The bytes the runner signs and posts for record i: {"data": R}, or {"data": {}} without result bytes."""
+        """The bytes the runner signs and posts for record i: {"data": R}, or {"data": {}} without result bytes; under
+        callback runners {"data": D}, D being the callback JSON the device wrote (R itself for task-queue records)."""
+        if self.cb_body_len is not None:
+            n = int(self.cb_body_len[i])
+            o = int(self.cb_body_off[i])
+            return b'{"data": ' + (self.payload[o:o + n].tobytes() if n else b"{}") + b"}"
         r = self.result(i)
         return b'{"data": ' + (r if r is not None else b"{}") + b"}"
+
+    def callback_url(self, i: int) -> Optional[str]:
+        """The task's own callback URL (a function task's callback_url kwarg), or None: the stub's URL."""
+        if self.cb_url_len is None or not int(self.cb_url_len[i]):
+            return None
+        o = int(self.cb_url_off[i])
+        return self.payload[o:o + int(self.cb_url_len[i])].tobytes().decode("utf-8")
 
     def callback_headers(self, i: int, status: Optional[str] = None) -> dict:
         """send_callback's headers for record i (status: the runner's TaskStatus, by default the record's)."""
@@ -214,6 +231,14 @@ class DeviceQueue:
             key = bytes(signing_key)
             self._check(self._lib.b9_set_callback_policy(self._ctx, 1, key if key else None, len(key)))
 
+    def set_callback_runners(self, function: bool = False, endpoint: bool = False) -> None:
+        """b9_set_callback_runners: under the callback policy, also settle the function runner's callbacks (pickle tasks of
+        full_pickle=True drains) and the endpoint runner's (endpoint=True drains) on the device. fetch(callbacks=True) then
+        carries each record's callback JSON and URL (callback_body, callback_url)."""
+        runners = (L.CB_RUNNER_FUNCTION if function else 0) | (L.CB_RUNNER_ENDPOINT if endpoint else 0)
+        self._check(self._lib.b9_set_callback_runners(self._ctx, runners))
+        self._cb_runners = runners
+
     def set_retry_policy(self, retry_for: Optional[Iterable[type]], max_retries: int) -> None:
         """b9_set_retry_policy: the stub's `retry_for` classes and TaskPolicy.MaxRetries. A task whose handler raised one of
         them comes back RETRY (and is pushed again, retries + 1, when its drain is fetched) or, once its retries reached
@@ -268,9 +293,18 @@ class DeviceQueue:
         kind = np.empty(max(n, 1), np.uint8)
         digest = np.empty((max(n, 1), 32), np.uint8)
         cb = L.Callbacks(kind.ctypes.data, digest.ctypes.data, max(n, 1), 0)
-        got = self._check(self._lib.b9_drain_fetch_callbacks(self._ctx, C.byref(r), C.byref(cb)))
+        if not getattr(self, "_cb_runners", 0):
+            got = self._check(self._lib.b9_drain_fetch_callbacks(self._ctx, C.byref(r), C.byref(cb)))
+            return DrainResult(ids[:got], status[:got], has[:got], off[:got], ln[:got], pl[:int(r.n_bytes)], int(r.n_popped), float(r.task_duration),
+                               kind[:got], digest[:got], int(cb.timestamp))
+        b_off = np.zeros(max(n, 1), np.uint64)
+        b_len = np.zeros(max(n, 1), np.uint32)
+        u_off = np.zeros(max(n, 1), np.uint64)
+        u_len = np.zeros(max(n, 1), np.uint32)
+        rq = L.CallbackRequests(b_off.ctypes.data, b_len.ctypes.data, u_off.ctypes.data, u_len.ctypes.data, max(n, 1))
+        got = self._check(self._lib.b9_drain_fetch_callback_requests(self._ctx, C.byref(r), C.byref(cb), C.byref(rq)))
         return DrainResult(ids[:got], status[:got], has[:got], off[:got], ln[:got], pl[:int(r.n_bytes)], int(r.n_popped), float(r.task_duration),
-                           kind[:got], digest[:got], int(cb.timestamp))
+                           kind[:got], digest[:got], int(cb.timestamp), b_off[:got], b_len[:got], u_off[:got], u_len[:got])
 
     def drain_object(self, handler: str, max_tasks: int = 1 << 22, endpoint: bool = False) -> np.ndarray:
         """One drain whose records land as ONE result-sink object (b9_drain_fetch_object): header + index + blob."""

@@ -32,11 +32,17 @@ class Endpoint:
 
     def __init__(self, cpu: Any = 1.0, memory: Any = 128, gpu: Any = "", image: Any = None, timeout: int = 180, workers: int = 1,
                  name: Optional[str] = None, gpu_handler: Optional[str] = None, device: int = 0,
-                 queue: Optional[DeviceQueue] = None, **kwargs: Any):
+                 queue: Optional[DeviceQueue] = None, callback_url: Optional[str] = None, signing_key: Optional[bytes] = None,
+                 **kwargs: Any):
         self.cpu, self.memory, self.gpu, self.image, self.timeout, self.workers = cpu, memory, gpu, image, timeout, workers
         self.name = name
         self.gpu_handler = gpu_handler or os.environ.get("B9_GPU_HANDLER", "identity")
         self.device = device
+        # the stub's callback URL: the device settles and signs the runner's callback of every answered request
+        # (b9_set_callback_runners), with the workspace's signing_key (None or b"": unsigned); nothing is posted here
+        self.callback_url = callback_url
+        self.signing_key = bytes(signing_key or b"")
+        self._cb_set = False
         self.extra = kwargs
         self._queue = queue
         self.stub_id = str(uuid.uuid4())
@@ -58,6 +64,9 @@ class _CallableWrapper:
         self.func = func
         self.parent = parent
         self.unsupported: List[bytes] = []        # request bodies the device did not answer (status UNSUPPORTED)
+        # with a callback_url: per body of the last call, what the runner hands requests.post, (url, body bytes, headers),
+        # or None (no task: a 400; or a callback left to the host, such as an ERROR's traceback)
+        self.callbacks: List[Optional[tuple]] = []
 
     def local(self, *args: Any, **kwargs: Any) -> Any:
         return self.func(*args, **kwargs)
@@ -79,9 +88,15 @@ class _CallableWrapper:
         q.flush()
         want = {tid: k for k, tid in enumerate(ids)}
         out: List[Optional[Tuple[Optional[int], Optional[bytes]]]] = [None] * len(bodies)
+        cb = bool(self.parent.callback_url)
+        if cb and not self.parent._cb_set:
+            q.set_callback_policy(self.parent.signing_key)
+            q.set_callback_runners(endpoint=True)
+            self.parent._cb_set = True
+        self.callbacks = [None] * len(bodies)
         seen = 0
         while seen < len(bodies):
-            r = q.drain(self.parent.gpu_handler, endpoint=True)
+            r = q.drain(self.parent.gpu_handler, endpoint=True, callbacks=cb)
             if r.n == 0:
                 break
             for i in range(r.n):
@@ -89,6 +104,8 @@ class _CallableWrapper:
                 if k is None:
                     continue
                 st = int(r.status[i])
+                if cb and int(r.cb_kind[i]) == L.CB_POST:
+                    self.callbacks[k] = (self.parent.callback_url, r.callback_body(i), r.callback_headers(i))
                 if st == L.ST_COMPLETE:
                     out[k] = (200, r.result(i))
                 elif st == L.ST_REJECTED:

@@ -35,12 +35,18 @@ class Function:
 
     def __init__(self, cpu: Any = 1.0, memory: Any = 128, gpu: Any = "", image: Any = None, timeout: int = 3600, retries: int = 3,
                  name: Optional[str] = None, headless: bool = False, gpu_handler: Optional[str] = None, device: int = 0,
-                 queue: Optional[DeviceQueue] = None, full_pickle: bool = False, **kwargs: Any):
+                 queue: Optional[DeviceQueue] = None, full_pickle: bool = False, callback_url: Optional[str] = None,
+                 signing_key: Optional[bytes] = None, **kwargs: Any):
         self.cpu, self.memory, self.gpu, self.image, self.timeout, self.retries = cpu, memory, gpu, image, timeout, retries
         self.name, self.headless = name, headless
         self.gpu_handler = gpu_handler or os.environ.get("B9_GPU_HANDLER", "identity")
         self.device = device
         self.full_pickle = full_pickle            # B9_DRAIN_PICKLE_FULL: every handler over plain values, not just one str
+        # the stub's callback URL: the device settles and signs the runner's callback of every completed task (full_pickle
+        # drains; b9_set_callback_runners), with the workspace's signing_key (None or b"": unsigned); nothing is posted here
+        self.callback_url = callback_url
+        self.signing_key = bytes(signing_key or b"")
+        self._cb_set = False
         self.extra = kwargs
         self._queue = queue
         self.stub_id = str(uuid.uuid4())
@@ -65,6 +71,9 @@ class _CallableWrapper:
         self.func = func
         self.parent = parent
         self.unsupported: List[Any] = []          # inputs whose pickle the device does not settle (status UNSUPPORTED)
+        # with a callback_url: per input of the last call, what the runner hands requests.post, (url, body bytes, headers),
+        # or None (nothing the device posts: an unsendable body, or a callback left to the host, such as an ERROR's)
+        self.callbacks: List[Optional[tuple]] = []
 
     def __call__(self, *args: Any, **kwargs: Any) -> Any:
         if os.environ.get("CONTAINER_ID") is not None:          # function.py:178-181: inside a container the call is local
@@ -103,15 +112,23 @@ class _CallableWrapper:
         q.push_batch(np.frombuffer(b"".join(ids), np.uint8).reshape(-1, 16), blob, offsets, flags=np.full(n, TF_PICKLE, np.uint8))
         want = {i: k for k, i in enumerate(ids)}
         out: List[Optional[Tuple[str, Optional[bytes]]]] = [None] * n
+        cb = bool(self.parent.callback_url)
+        if cb and not self.parent._cb_set:
+            q.set_callback_policy(self.parent.signing_key)
+            q.set_callback_runners(function=True)
+            self.parent._cb_set = True
+        self.callbacks = [None] * n
         seen = 0
         while seen < n:
-            r = q.drain(self.parent.gpu_handler, full_pickle=self.parent.full_pickle)
+            r = q.drain(self.parent.gpu_handler, full_pickle=self.parent.full_pickle, callbacks=cb)
             if r.n == 0:
                 break
             for i in range(r.n):
                 k = want.get(r.task_ids[i].tobytes())
                 if k is not None:
                     out[k] = (STATUS_NAMES[int(r.status[i])], r.result(i))
+                    if cb and int(r.cb_kind[i]) == L.CB_POST:
+                        self.callbacks[k] = (r.callback_url(i) or self.parent.callback_url, r.callback_body(i), r.callback_headers(i))
                     seen += 1
         return [o if o is not None else ("ERROR", None) for o in out]
 

@@ -340,7 +340,7 @@ enum b9_callback_kind { B9_CB_NONE = 0, B9_CB_POST = 1, B9_CB_UNSENDABLE = 2, B9
  * (SignPayload answers Ok: false): the runner still posts, with X-Task-Signature "" and X-Task-Timestamp 0, so the pass
  * writes no digests and reports timestamp 0. A key longer than 64 bytes is hashed first, as Go's hmac.New does. Applies to
  * the b9_drain_launch calls made after it (a drain-side call); enabled = 0, the default, launches exactly what a drain
- * without a policy launches. Not affected: b9_endpoint_drain_launch. Returns 0, or B9_EINVAL (NULL ctx, NULL key with
+ * without a policy launches. Not affected: b9_endpoint_drain_launch (unless b9_set_callback_runners). Returns 0, or B9_EINVAL (NULL ctx, NULL key with
  * key_len > 0), B9_ENOMEM. Added without an ABI version change: probe for it with dlsym. */
 int      b9_set_callback_policy(b9_ctx *ctx, int enabled, const uint8_t *signing_key, uint32_t key_len);
 typedef struct b9_callbacks {
@@ -354,6 +354,48 @@ typedef struct b9_callbacks {
  * consumed when either the results or `cb` are too small). B9_EINVAL when the fetched launch ran no callback pass (no
  * policy, b9_endpoint_drain_launch, the wire encoders). After a burst of B9_DRAIN_ASYNC launches, the last one's. */
 int64_t  b9_drain_fetch_callbacks(b9_ctx *ctx, b9_results *out, b9_callbacks *cb);
+
+/* ---- the function and endpoint runners' callbacks ----------------------------------------------------------------------
+ * Both runners end in the same send_callback (runner/common.py:406-481): POST {"data": payload} to
+ * `override_callback_url or the stub's URL`, signed over json.dumps(body) with its defaults (", " / ": " separators,
+ * ensure_ascii=True), posted by requests with allow_nan=False. Their records are not that JSON (a cloudpickle of the
+ * result; a compact ensure_ascii=False JSONResponse body), so under a runner's bit the device writes each callback's JSON
+ * D as well, and signs {"data": D}. Per record:
+ *   function (B9_TF_PICKLE records of b9_drain_launch(..., B9_DRAIN_PICKLE_FULL); runner/function.py:235-343):
+ *     B9_CB_POST        COMPLETE with a value json.dumps writes, every float finite, every int within int64: D =
+ *                       json.dumps(result) (None -> null; no `or {}`). URL: the task's kwargs["callback_url"] when it is a
+ *                       truthy str, else the stub's (url length 0).
+ *     B9_CB_UNSENDABLE  COMPLETE with bytes anywhere in the value (json.dumps raises, nothing is signed), or a NaN /
+ *                       Infinity value or float key (signed, then refused by requests). No D, digest zero.
+ *     B9_CB_HOST        COMPLETE with an int outside int64, a truthy callback_url that is not a str or holds a surrogate,
+ *                       or a D longer than 1 MiB (the walk stops there: bytes or a non-finite float that come later in
+ *                       the value leave the record HOST, not UNSENDABLE); ERROR (its body holds the exception text),
+ *                       UNSUPPORTED; every pickle record of a launch without B9_DRAIN_PICKLE_FULL.
+ *   endpoint (b9_endpoint_drain_launch; middleware.py:29-78): COMPLETE -> B9_CB_POST with D = the record E re-spaced
+ *     (", " / ": " outside strings) and with every non-ASCII code point and DEL inside strings as \uXXXX; the stub's URL.
+ *     REJECTED -> B9_CB_NONE (no task exists); ERROR, UNSUPPORTED -> B9_CB_HOST.
+ * Task-queue records keep the rules above, with D = R (or `{}` without result bytes). */
+#define B9_CB_RUNNER_FUNCTION 0x1u   /* settle B9_TF_PICKLE records of b9_drain_launch(..., B9_DRAIN_PICKLE_FULL)        */
+#define B9_CB_RUNNER_ENDPOINT 0x2u   /* run the callback pass after b9_endpoint_drain_launch                            */
+/* Which runners' callbacks the device settles under a callback policy (b9_set_callback_policy; without one, nothing
+ * changes). Default 0: every launch enqueues and answers exactly as without this call. Applies to the launches made after
+ * it (a drain-side call). Returns 0, or B9_EINVAL (NULL ctx, other bits), B9_ENOMEM. Probe for it with dlsym. */
+int      b9_set_callback_runners(b9_ctx *ctx, uint32_t runners);
+typedef struct b9_callback_requests {
+    uint64_t *body_offsets;  /* [cap_tasks] D of record i = b9_results.payload[body_offsets[i], +body_lengths[i]) */
+    uint32_t *body_lengths;  /*             0: D is `{}` (task-queue records without result bytes; no request)   */
+    uint64_t *url_offsets;   /* [cap_tasks] the task's own callback URL (UTF-8) in b9_results.payload            */
+    uint32_t *url_lengths;   /*             0: post to the stub's URL                                            */
+    uint32_t  cap_tasks;
+} b9_callback_requests;
+/* b9_drain_fetch_callbacks plus each record's D and URL, in the same read-back, commit and B9_ENOSPC (rq->cap_tasks too
+ * small consumes nothing). D and URL bytes are reserved from the drain's result bytes like its records, so n_bytes /
+ * need_bytes count them; the records' own offsets, lengths and bytes are as without them. The body to post and sign is
+ * `{"data": ` + D + `}`. B9_EINVAL when the fetched launch ran no callback pass, as b9_drain_fetch_callbacks. When a
+ * launch ran a runner's pass (a function-runner launch with pickle tasks in its window, an endpoint launch), its digests
+ * sign D, not the records: b9_drain_fetch_callbacks refuses such a launch (B9_EINVAL, nothing consumed) and this fetch is
+ * the one that gives the signed bodies. */
+int64_t  b9_drain_fetch_callback_requests(b9_ctx *ctx, b9_results *out, b9_callbacks *cb, b9_callback_requests *rq);
 
 /* ---- consumer side ---------------------------------------------------------------------------
  * b9_drain replaces, for up to max_tasks pending tasks in FIFO order, the whole
