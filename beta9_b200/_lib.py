@@ -10,6 +10,7 @@ SO = os.environ.get("B9GPU_LIB") or os.path.join(PKG, "libb9gpu.so")     # B9GPU
 
 B9_OK, B9_EINVAL, B9_ENOMEM, B9_ENOSPC, B9_E2BIG, B9_EIO, B9_ENODEV, B9_ENOSYS, B9_ENOENT = 0, -22, -12, -28, -7, -5, -19, -38, -2
 H_IDENTITY, H_CRC32, H_VADD_F32, H_JSON_SUM = 0, 1, 2, 3
+H_USER_BASE = 256                                                      # ids of b9_handler_load's handlers start here
 ST_COMPLETE, ST_ERROR, ST_RETRY, ST_REJECTED, ST_UNSUPPORTED, ST_RETRY_LIMIT = 0, 1, 2, 3, 4, 5
 # B9_EXC_*: the exception class a device handler raised, for b9_set_retry_policy
 EXC_TYPE_ERROR, EXC_ATTRIBUTE_ERROR, EXC_UNICODE_ENCODE, EXC_KEY_ERROR, EXC_VALUE_ERROR, EXC_BINASCII_ERROR = 0x01, 0x02, 0x04, 0x08, 0x10, 0x20
@@ -81,6 +82,7 @@ SYMBOLS = {
     "b9_last_error": (C.c_char_p, [C.c_void_p]),
     "b9_handler_name": (C.c_char_p, [C.c_int]),
     "b9_handler_id": (C.c_int, [C.c_char_p]),
+    "b9_handler_load": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_char_p, C.POINTER(C.c_int32)]),
     "b9_host_alloc": (C.c_void_p, [C.c_void_p, C.c_uint64]),
     "b9_host_free": (None, [C.c_void_p, C.c_void_p]),
     "b9_batch_push": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(PushMeta)]),

@@ -9,7 +9,7 @@ from __future__ import annotations
 import os
 import subprocess
 import sys
-from typing import List
+from typing import List, Optional
 
 PKG = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(PKG)
@@ -56,6 +56,46 @@ def build(force: bool = False, verbose_ptxas: bool = False) -> str:
     return SO
 
 
+HANDLER_FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-cubin", "-gencode", "arch=compute_90a,code=sm_90a"]
+EXAMPLE_HANDLERS = os.path.join(ROOT, "examples", "handlers", "handlers.cu")
+EXAMPLE_CUBIN = os.path.join(PKG, "example_handlers.cubin")     # build product (git-ignored), loaded with b9_handler_load
+
+
+def handler_abi_version() -> int:
+    """B9_HANDLER_ABI_VERSION (drain_kernel.cuh): the version the entry names of a handler image carry."""
+    import re
+    with open(os.path.join(CSRC, "drain_kernel.cuh")) as f:
+        return int(re.search(r"#define B9_HANDLER_ABI_VERSION (\d+)", f.read()).group(1))
+
+
+def compile_handlers(src: str, out: str, includes: Optional[List[str]] = None, force: bool = False) -> str:
+    """Compiles a translation unit of B9_HANDLER lines (include/b9gpu_handler.cuh) to an sm_90a cubin for
+    b9_handler_load, with the library's flags and include path. As build(): nothing is done while `out` is newer than
+    `src`, the headers next to it and the library's device headers."""
+    src, out = os.path.abspath(src), os.path.abspath(out)
+    here = os.path.dirname(src)
+    deps = [src] + _deps() + [os.path.join(ROOT, "include", "b9gpu_handler.cuh")] + \
+        [os.path.join(here, f) for f in os.listdir(here) if f.endswith((".cuh", ".h"))]
+    if not force and os.path.exists(out) and not any(os.path.getmtime(d) > os.path.getmtime(out) for d in deps):
+        return out
+    if not os.path.exists(NVCC):
+        raise RuntimeError(f"nvcc not found at {NVCC}: {src} cannot be compiled")
+    inc = ["-I" + os.path.join(ROOT, "include"), "-I" + here] + ["-I" + d for d in (includes or [])]
+    tmp = out + ".tmp"
+    r = subprocess.run([NVCC] + HANDLER_FLAGS + inc + ["-o", tmp, src], capture_output=True, text=True)
+    if r.returncode:
+        if os.path.exists(tmp):
+            os.remove(tmp)
+        raise RuntimeError("nvcc failed:\n" + r.stdout + r.stderr)
+    os.replace(tmp, out)
+    return out
+
+
+def build_examples(force: bool = False) -> str:
+    """The example handlers (examples/handlers) as beta9_b200/example_handlers.cubin, so that runs need no nvcc."""
+    return compile_handlers(EXAMPLE_HANDLERS, EXAMPLE_CUBIN, force=force)
+
+
 def build_variant(name: str, defines: List[str]) -> str:
     """An alternative build for A/B timing on one box: ab_builds/<name>.so compiled with extra -D switches
     (selected at run time with B9GPU_LIB=...). ab_builds/ is git-ignored."""
@@ -75,3 +115,4 @@ if __name__ == "__main__":
         print(build_variant(sys.argv[i + 1], [a[2:] for a in sys.argv[i + 2:] if a.startswith("-D")]))
         sys.exit(0)
     print(build(force="--force" in sys.argv, verbose_ptxas="--ptxas-v" in sys.argv))
+    print(build_examples(force="--force" in sys.argv))

@@ -52,6 +52,7 @@ cudaError_t launch_callback_sign(const void* args, size_t args_size, const uint3
 // = ENDPOINT_TILE_TASKS and n_tiles set for it
 cudaError_t launch_endpoint_drain(const void* args, size_t args_size, int handler, int sm_count, cudaStream_t s);
 constexpr uint32_t ENDPOINT_TILE_TASKS = 32;   // endpoint_drain.cu's EP_TILE (the launcher refuses any other)
+constexpr int USER_DRAIN_WARPS = 4;            // user_drain.cuh's UD_WARPS (its tiles are ENDPOINT_TILE_TASKS slots too)
 // the function runner's callback pass (in place of the pickle pass, behind callback_sign_kernel) or the endpoint runner's
 // (behind endpoint_drain_kernel), from callback_runners.cu; out: kind, digest, body_off, body_len, url_off, url_len
 cudaError_t launch_callback_runner(int endpoint, const void* args, size_t args_size, int handler, const uint32_t mid[16], int keyed,
@@ -176,6 +177,13 @@ struct WaitingResults {
     uint32_t async_n = 0; uint64_t async_in_bytes = 0;
 };
 
+// A handler image loaded with b9_handler_load: its two B9_HANDLER entry points (b9gpu_handler.cuh) and their residency
+struct UserHandler {
+    cudaLibrary_t lib = nullptr;
+    cudaKernel_t tq = nullptr, ep = nullptr;   // the task-queue and the endpoint drain
+    int per_sm_tq = 1, per_sm_ep = 1;          // resident CTAs per SM
+};
+
 }  // namespace
 
 struct b9_ctx {
@@ -260,9 +268,13 @@ struct b9_ctx {
 
     b9_stats stats{};
 
-    // what the members do not release themselves: the segment events and the submission arenas' page-locked memory
-    // (submit_buffer.h builds without CUDA)
+    // handler images of b9_handler_load (under out_mu): id B9_H_USER_BASE + k is users[k]
+    std::vector<UserHandler> users;
+
+    // what the members do not release themselves: the segment events, the submission arenas' page-locked memory
+    // (submit_buffer.h builds without CUDA) and the handler images
     ~b9_ctx() {
+        for (const UserHandler& u : users) cudaLibraryUnload(u.lib);
         for (const Segment& sg : segs) cudaEventDestroy(sg.ready);
         for (cudaEvent_t e : event_pool) cudaEventDestroy(e);
         if (sb) for (SubmitArena& A : sb->arena) {
@@ -752,6 +764,78 @@ int b9_handler_id(const char* name) {
     return B9_ENOSYS;
 }
 
+// The length an image's own header gives it, checked against `size`: an ELF64 cubin whose header tables and sections lie
+// within `size`, or a fatbin whose header and payload do. 0: neither, or truncated. (cudaLibraryLoadData takes no size:
+// it reads what the header says, so the header is checked first.)
+static uint64_t image_bytes(const uint8_t* b, uint64_t size) {
+    if (size >= 64 && memcmp(b, "\x7f" "ELF", 4) == 0 && b[4] == 2) {                       // ELFCLASS64
+        uint64_t phoff, shoff; uint16_t phentsize, phnum, shentsize, shnum;
+        memcpy(&phoff, b + 0x20, 8); memcpy(&shoff, b + 0x28, 8);
+        memcpy(&phentsize, b + 0x36, 2); memcpy(&phnum, b + 0x38, 2); memcpy(&shentsize, b + 0x3A, 2); memcpy(&shnum, b + 0x3C, 2);
+        if (phoff > size || (uint64_t)phentsize * phnum > size - phoff) return 0;
+        if (shoff > size || shentsize < 64 || (uint64_t)shentsize * shnum > size - shoff) return 0;
+        uint64_t end = std::max<uint64_t>(phoff + (uint64_t)phentsize * phnum, shoff + (uint64_t)shentsize * shnum);
+        for (uint32_t k = 0; k < shnum; ++k) {
+            const uint8_t* sh = b + shoff + (uint64_t)k * shentsize;
+            uint32_t type; uint64_t off, sz;
+            memcpy(&type, sh + 4, 4); memcpy(&off, sh + 0x18, 8); memcpy(&sz, sh + 0x20, 8);
+            if (type == 8) continue;                                                          // SHT_NOBITS
+            if (off > size || sz > size - off) return 0;
+            end = std::max<uint64_t>(end, off + sz);
+        }
+        return end;
+    }
+    uint32_t magic = 0;
+    if (size >= 16) memcpy(&magic, b, 4);
+    if (magic == 0xBA55ED50u) {                                                               // fatbin: magic, version, header size, payload size
+        uint16_t hs; uint64_t fs;
+        memcpy(&hs, b + 6, 2); memcpy(&fs, b + 8, 8);
+        if (hs < 16 || fs > size || hs > size - fs) return 0;
+        return hs + fs;
+    }
+    return 0;
+}
+
+int b9_handler_load(b9_ctx* c, const void* image, uint64_t size, const char* name, int32_t* handler_out) {
+    if (!c || !image || !name || !handler_out) return fail(B9_EINVAL, "b9_handler_load: NULL argument");
+    const size_t nl = strlen(name);
+    bool ident = nl > 0 && nl <= 200 && !(name[0] >= '0' && name[0] <= '9');
+    for (size_t k = 0; k < nl && ident; ++k) ident = name[k] == '_' || (name[k] >= '0' && name[k] <= '9') || ((name[k] | 0x20) >= 'a' && (name[k] | 0x20) <= 'z');
+    if (!ident) return fail(B9_EINVAL, "b9_handler_load: \"%.64s\" is not a B9_HANDLER name (a C identifier)", name);
+    if (!image_bytes((const uint8_t*)image, size))
+        return fail(B9_EINVAL, "b9_handler_load: the image is not an ELF cubin or a fatbin that fits in %llu bytes", (unsigned long long)size);
+    OutLock out_lk(c);
+    CU(cudaSetDevice(c->device));
+    UserHandler u;
+    cudaError_t e = cudaLibraryLoadData(&u.lib, image, nullptr, nullptr, 0, nullptr, nullptr, 0);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        return fail(B9_EINVAL, "b9_handler_load: the image does not load on device %d: %s", c->device, cudaGetErrorString(e));
+    }
+    char tq[256], ep[256];
+    snprintf(tq, sizeof tq, "b9h_v%d_tq_%s", B9_HANDLER_ABI_VERSION, name);
+    snprintf(ep, sizeof ep, "b9h_v%d_ep_%s", B9_HANDLER_ABI_VERSION, name);
+    e = cudaLibraryGetKernel(&u.tq, u.lib, tq);
+    if (e == cudaSuccess) e = cudaLibraryGetKernel(&u.ep, u.lib, ep);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        cudaLibraryUnload(u.lib);
+        return fail(B9_EINVAL, "b9_handler_load: the image has no entry %s / %s: it holds no B9_HANDLER(%s, ...), or it was built "
+                               "against another handler ABI version than this library's %d (B9_HANDLER_ABI_VERSION)", tq, ep, name, B9_HANDLER_ABI_VERSION);
+    }
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&u.per_sm_tq, (const void*)u.tq, USER_DRAIN_WARPS * 32, 0);
+    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&u.per_sm_ep, (const void*)u.ep, USER_DRAIN_WARPS * 32, 0);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        cudaLibraryUnload(u.lib);
+        return fail(B9_EINVAL, "b9_handler_load: %s: %s", tq, cudaGetErrorString(e));
+    }
+    u.per_sm_tq = std::max(u.per_sm_tq, 1); u.per_sm_ep = std::max(u.per_sm_ep, 1);
+    c->users.push_back(u);
+    *handler_out = B9_H_USER_BASE + (int32_t)(c->users.size() - 1);
+    return B9_OK;
+}
+
 int b9_ctx_create(const b9_opts* opts, b9_ctx** out) {
     if (!out) return fail(B9_EINVAL, "b9_ctx_create: out is NULL");
     *out = nullptr;
@@ -1215,6 +1299,14 @@ static int finish_launch(b9_ctx* c) {
 // endpoint runner's responses) instead of drain3_kernel (the task-queue runner's results).
 static int64_t drain_launch_common(b9_ctx* c, int handler, uint32_t max_tasks, int peek, bool endpoint) {
     std::lock_guard<std::mutex> out_lk(c->out_mu);
+    // a user handler (b9_handler_load): an id this context returned, and not with the function path's pass
+    const UserHandler* user = nullptr;
+    if (handler >= B9_H_USER_BASE) {
+        if ((size_t)(handler - B9_H_USER_BASE) >= c->users.size())
+            return fail(B9_ENOSYS, "%s: unknown handler %d (not loaded into this context)", endpoint ? "b9_endpoint_drain_launch" : "b9_drain_launch", handler);
+        if (peek & B9_DRAIN_PICKLE_FULL) return fail(B9_EINVAL, "b9_drain_launch: B9_DRAIN_PICKLE_FULL does not apply to a user handler (%d)", handler);
+        user = &c->users[handler - B9_H_USER_BASE];
+    }
     CU(cudaSetDevice(c->device));
     // results of an earlier launch that were never fetched are dropped; their tasks are still
     // pending (a pop is committed by a successful fetch, never by a launch). (An open burst of async launches stays open.)
@@ -1293,15 +1385,27 @@ static int64_t drain_launch_common(b9_ctx* c, int handler, uint32_t max_tasks, i
     c->last_op_drain = false;
     cudaError_t le;
     uint32_t tt = 0;
-    if (endpoint) {
-        // never a programmatic dependent, and the next drain3_kernel is not launched as its dependent either: the timed
-        // span ends right behind it (end_drain_span below), which leaves last_op_drain false. The kernel zeroes the next
-        // control block itself, as drain3_kernel does (endpoint_drain.cu).
+    if (endpoint || user) {
+        // the endpoint drain and a user handler's drains (user_drain.cuh, either rendering) have one shape: 32-slot tiles,
+        // one task per lane. Never a programmatic dependent, and the next drain3_kernel is not launched as its dependent
+        // either: the timed span ends right behind it (end_drain_span below), which leaves last_op_drain false. The kernel
+        // zeroes the next control block itself, as drain3_kernel does (endpoint_drain.cu).
         a.tile_tasks = ENDPOINT_TILE_TASKS;
         a.n_tiles = (n + ENDPOINT_TILE_TASKS - 1) / ENDPOINT_TILE_TASKS;
+        tt = ENDPOINT_TILE_TASKS;                                           // (the callback sign pass's record indices)
         le = a.count_mode ? launch_tile_counts(a, ENDPOINT_TILE_TASKS, s) : cudaSuccess;
-        if (le == cudaSuccess) le = launch_endpoint_drain(&a, sizeof a, handler, c->sm_count, s);
-        if (le != cudaSuccess) { c->ctl_dirty = true; return fail(B9_EIO, "endpoint drain kernel launch failed: %s", cudaGetErrorString(le)); }
+        if (le == cudaSuccess && !user) le = launch_endpoint_drain(&a, sizeof a, handler, c->sm_count, s);
+        else if (le == cudaSuccess) {
+            const uint64_t ctas_needed = ((uint64_t)a.n_tiles + USER_DRAIN_WARPS - 1) / USER_DRAIN_WARPS;
+            const uint64_t resident = (uint64_t)(endpoint ? user->per_sm_ep : user->per_sm_tq) * (uint64_t)c->sm_count;
+            const uint32_t ctas = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(ctas_needed, resident));
+            void* args[] = {&a};
+            le = cudaLaunchKernel((const void*)(endpoint ? user->ep : user->tq), dim3(ctas), dim3(USER_DRAIN_WARPS * 32), args, 0, s);
+        }
+        if (le != cudaSuccess) {
+            c->ctl_dirty = true;
+            return fail(B9_EIO, "%s drain kernel launch failed: %s", user ? "user handler" : "endpoint", cudaGetErrorString(le));
+        }
         c->last_op_drain = true;
         c->burst_open = true;
         if (!c->res.cb) end_drain_span(c);                                  // (with the runner's callback pass: behind that)
@@ -1311,7 +1415,7 @@ static int64_t drain_launch_common(b9_ctx* c, int handler, uint32_t max_tasks, i
     case B9_H_VADD_F32: le = launch_drain3<2>(a, in_bytes / n, win_max_len, c->stage_bytes_override, c->sm_count, overlap, s, &grid, &tt); break;
     default:            le = launch_drain3<3>(a, in_bytes / n, win_max_len, c->stage_bytes_override, c->sm_count, overlap, s, &grid, &tt); break;
     }
-    if (!endpoint) {
+    if (!endpoint && !user) {
         if (le != cudaSuccess) { c->ctl_dirty = true; return fail(B9_EIO, "drain kernel launch failed: %s", cudaGetErrorString(le)); }
         c->last_op_drain = true;
         c->burst_open = true;
@@ -1364,13 +1468,13 @@ static int64_t drain_launch_common(b9_ctx* c, int handler, uint32_t max_tasks, i
 
 int64_t b9_drain_launch(b9_ctx* c, int handler, uint32_t max_tasks, int peek) {
     if (!c) return fail(B9_EINVAL, "b9_drain_launch: ctx is NULL");
-    if (handler < 0 || handler >= B9_H_COUNT_) return fail(B9_ENOSYS, "b9_drain_launch: unknown handler %d", handler);
+    if (handler < 0 || (handler >= B9_H_COUNT_ && handler < B9_H_USER_BASE)) return fail(B9_ENOSYS, "b9_drain_launch: unknown handler %d", handler);
     return drain_launch_common(c, handler, max_tasks, peek, false);
 }
 
 int64_t b9_endpoint_drain_launch(b9_ctx* c, int handler, uint32_t max_tasks, int flags) {
     if (!c) return fail(B9_EINVAL, "b9_endpoint_drain_launch: ctx is NULL");
-    if (handler < 0 || handler >= B9_H_COUNT_) return fail(B9_ENOSYS, "b9_endpoint_drain_launch: unknown handler %d", handler);
+    if (handler < 0 || (handler >= B9_H_COUNT_ && handler < B9_H_USER_BASE)) return fail(B9_ENOSYS, "b9_endpoint_drain_launch: unknown handler %d", handler);
     if (flags & ~(B9_DRAIN_PEEK | B9_DRAIN_ASYNC)) return fail(B9_EINVAL, "b9_endpoint_drain_launch: unknown flag bits 0x%x", flags);
     return drain_launch_common(c, handler, max_tasks, flags, true);
 }

@@ -137,6 +137,14 @@ struct DrainArgs {
                                     // (drain3_kernel<H, true>: the launch with a policy; <H, false> is the drain without one)
 };
 
+// The user-handler ABI (b9_handler_load, include/b9gpu_handler.cuh): a handler image's entry points receive this
+// DrainArgs (with its DrainOut and DrainCtl) by value, and their names carry this version, so that an image built against
+// another layout has no entry this library looks up. Bump the version with any change to those structs: the assert below
+// fails until the size it names is updated together with it.
+#define B9_HANDLER_ABI_VERSION 1
+static_assert(B9_HANDLER_ABI_VERSION == 1 && sizeof(DrainArgs) == 208 && sizeof(DrainOut) == 72 && sizeof(DrainCtl) == 48,
+              "DrainArgs / DrainOut / DrainCtl changed: bump B9_HANDLER_ABI_VERSION and the sizes here");
+
 // The status record j (of window task t) is written with: an ERROR whose exception class the retry policy names becomes
 // RETRY while the task's retries are below max_retries, else RETRY_LIMIT (Dispatcher.RetryTask's test,
 // pkg/task/dispatch.go:232-285). `value` is rec.value: an ERROR's exception class. t == ~0u: task_of[j] holds the task.

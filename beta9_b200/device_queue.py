@@ -8,9 +8,10 @@ from __future__ import annotations
 
 import binascii
 import ctypes as C
+import os
 import uuid
 from dataclasses import dataclass
-from typing import Iterable, List, Optional, Tuple
+from typing import Iterable, List, Optional, Tuple, Union
 
 import numpy as np
 
@@ -139,6 +140,7 @@ class DeviceQueue:
         self._ctx = ctx
         self.device = device
         self._res_bufs = None
+        self._user_handlers = {}                   # name -> id of the handlers load_handler loaded into this context
 
     def close(self) -> None:
         if getattr(self, "_ctx", None):
@@ -246,20 +248,42 @@ class DeviceQueue:
         (a task's retries are one byte); a larger value raises B9Error (B9_EINVAL)."""
         self._check(self._lib.b9_set_retry_policy(self._ctx, retry_mask(retry_for), max(0, int(max_retries))))
 
+    # ---- user handlers
+    def load_handler(self, image: Union[bytes, str, os.PathLike], name: str) -> int:
+        """b9_handler_load: loads the B9_HANDLER `name` of an sm_90a cubin or fatbin (its bytes, or a path to it) compiled
+        against include/b9gpu_handler.cuh (build.compile_handlers). Returns its id (H_USER_BASE + k); drains then take
+        `name` or the id wherever they take a built-in handler's name."""
+        if not isinstance(image, (bytes, bytearray, memoryview)):
+            with open(image, "rb") as f:
+                image = f.read()
+        data = bytes(image)
+        hid = C.c_int32(0)
+        self._check(self._lib.b9_handler_load(self._ctx, data, len(data), name.encode(), C.byref(hid)))
+        self._user_handlers[name] = int(hid.value)
+        return int(hid.value)
+
+    def handler_id(self, handler: Union[str, int]) -> int:
+        """The id of a built-in handler's name, of a name load_handler loaded, or an id as it is."""
+        if isinstance(handler, int):
+            return handler
+        if handler in self._user_handlers:
+            return self._user_handlers[handler]
+        return HANDLERS[handler]
+
     # ---- consumer side
-    def drain(self, handler: str, max_tasks: int = 1 << 22, cap_bytes: Optional[int] = None, full_pickle: bool = False,
+    def drain(self, handler: Union[str, int], max_tasks: int = 1 << 22, cap_bytes: Optional[int] = None, full_pickle: bool = False,
               endpoint: bool = False, callbacks: bool = False) -> DrainResult:
         """full_pickle=True (B9_DRAIN_PICKLE_FULL): pickle-framed tasks of every handler over plain values (include/b9gpu.h).
         endpoint=True (b9_endpoint_drain_launch): B9_TF_HTTP_BODY tasks answered with the endpoint runner's response bodies.
         callbacks=True (b9_drain_fetch_callbacks, under set_callback_policy): the result carries each record's callback."""
-        n = self._launch(HANDLERS[handler], max_tasks, L.DRAIN_PICKLE_FULL if full_pickle else 0, endpoint)
+        n = self._launch(self.handler_id(handler), max_tasks, L.DRAIN_PICKLE_FULL if full_pickle else 0, endpoint)
         return self._fetch(n, cap_bytes, callbacks)
 
-    def drain_launch(self, handler: str, max_tasks: int = 1 << 22, peek: bool = False, wait: bool = True, full_pickle: bool = False,
+    def drain_launch(self, handler: Union[str, int], max_tasks: int = 1 << 22, peek: bool = False, wait: bool = True, full_pickle: bool = False,
                      endpoint: bool = False) -> int:
         """wait=False (B9_DRAIN_ASYNC): returns once the kernels are enqueued; `sync()` or `fetch()` completes it."""
         flags = (1 if peek else 0) | (0 if wait else 2) | (L.DRAIN_PICKLE_FULL if full_pickle else 0)
-        return self._launch(HANDLERS[handler], max_tasks, flags, endpoint)
+        return self._launch(self.handler_id(handler), max_tasks, flags, endpoint)
 
     def _launch(self, h: int, max_tasks: int, flags: int, endpoint: bool) -> int:
         if not endpoint:
@@ -306,9 +330,9 @@ class DeviceQueue:
         return DrainResult(ids[:got], status[:got], has[:got], off[:got], ln[:got], pl[:int(r.n_bytes)], int(r.n_popped), float(r.task_duration),
                            kind[:got], digest[:got], int(cb.timestamp), b_off[:got], b_len[:got], u_off[:got], u_len[:got])
 
-    def drain_object(self, handler: str, max_tasks: int = 1 << 22, endpoint: bool = False) -> np.ndarray:
+    def drain_object(self, handler: Union[str, int], max_tasks: int = 1 << 22, endpoint: bool = False) -> np.ndarray:
         """One drain whose records land as ONE result-sink object (b9_drain_fetch_object): header + index + blob."""
-        self._launch(HANDLERS[handler], max_tasks, 0, endpoint)
+        self._launch(self.handler_id(handler), max_tasks, 0, endpoint)
         need = C.c_uint64(0)
         probe = np.zeros(128, np.uint8)
         rc = self._lib.b9_drain_fetch_object(self._ctx, probe.ctypes.data, 0, C.byref(need))      # B9_ENOSPC: tells the size, consumes nothing
@@ -318,9 +342,9 @@ class DeviceQueue:
         self._check(self._lib.b9_drain_fetch_object(self._ctx, obj.ctypes.data, obj.size, C.byref(need)))
         return obj
 
-    def drain_into(self, handler: str, max_tasks: int, res: "L.Results") -> int:
+    def drain_into(self, handler: Union[str, int], max_tasks: int, res: "L.Results") -> int:
         """b9_drain straight into caller-owned (ideally pinned) buffers described by `res`."""
-        return self._check(self._lib.b9_drain(self._ctx, HANDLERS[handler], max_tasks, C.byref(res)))
+        return self._check(self._lib.b9_drain(self._ctx, self.handler_id(handler), max_tasks, C.byref(res)))
 
     def wire_encode(self, workspace_name: str, stub_id: str, max_tasks: int = 1 << 22, executor: str = "taskqueue",
                     max_retries: int = 3, timeout: int = 3600, ttl: int = 7200, full: bool = False) -> DrainResult:

@@ -18,7 +18,7 @@ from __future__ import annotations
 
 import os
 import uuid
-from typing import Any, Callable, List, Optional, Sequence, Tuple
+from typing import Any, Callable, List, Optional, Sequence, Tuple, Union
 
 from . import _lib as L
 from .device_queue import DeviceQueue
@@ -32,11 +32,15 @@ class Endpoint:
 
     def __init__(self, cpu: Any = 1.0, memory: Any = 128, gpu: Any = "", image: Any = None, timeout: int = 180, workers: int = 1,
                  name: Optional[str] = None, gpu_handler: Optional[str] = None, device: int = 0,
+                 gpu_handler_image: Optional[Union[bytes, str]] = None,
                  queue: Optional[DeviceQueue] = None, callback_url: Optional[str] = None, signing_key: Optional[bytes] = None,
                  **kwargs: Any):
         self.cpu, self.memory, self.gpu, self.image, self.timeout, self.workers = cpu, memory, gpu, image, timeout, workers
         self.name = name
         self.gpu_handler = gpu_handler or os.environ.get("B9_GPU_HANDLER", "identity")
+        # a user handler (b9gpu_handler.cuh): the sm_90a image (bytes or a path) that holds B9_HANDLER(gpu_handler, ...)
+        self.gpu_handler_image = gpu_handler_image or os.environ.get("B9_GPU_HANDLER_IMAGE") or None
+        self._handler_loaded = False
         self.device = device
         # the stub's callback URL: the device settles and signs the runner's callback of every answered request
         # (b9_set_callback_runners), with the workspace's signing_key (None or b"": unsigned); nothing is posted here
@@ -51,6 +55,9 @@ class Endpoint:
     def queue(self) -> DeviceQueue:
         if self._queue is None:
             self._queue = DeviceQueue(device=self.device)     # raises without a GPU: no CPU path
+        if self.gpu_handler_image is not None and not self._handler_loaded:
+            self._queue.load_handler(self.gpu_handler_image, self.gpu_handler)
+            self._handler_loaded = True
         return self._queue
 
     def __call__(self, func: Callable) -> "_CallableWrapper":

@@ -48,7 +48,8 @@ class Task:
 
 class TaskQueue:
     """Decorator. Resource arguments are accepted and kept for API compatibility; only the ones
-    this path reads have an effect (`max_pending_tasks`, `retries`, `retry_for`, `gpu_handler`, `device`). A task whose
+    this path reads have an effect (`max_pending_tasks`, `retries`, `retry_for`, `gpu_handler`, `gpu_handler_image`,
+    `device`). A task whose
     handler raises a class in `retry_for` (an exact match, as the runner's retry_on_errors) comes back "RETRY" and is
     queued again, up to `retries` times; after that it comes back "RETRY_LIMIT" (the gateway cancels it). With
     `callback_url`, every drained task carries the callback the runner would post (Task.callback), signed with the
@@ -58,6 +59,7 @@ class TaskQueue:
                  timeout: int = 3600, retries: int = 3, workers: int = 1, keep_warm_seconds: int = 10,
                  max_pending_tasks: int = DEFAULT_MAX_PENDING_TASKS, name: Optional[str] = None,
                  retry_for: Optional[List[type]] = None, gpu_handler: Optional[str] = None, device: int = 0, queue: Optional[DeviceQueue] = None,
+                 gpu_handler_image: Optional[Union[bytes, str]] = None,
                  callback_url: Optional[str] = None, signing_key: Optional[bytes] = None, **kwargs: Any):
         self.cpu = int(float(cpu) * 1000) if not isinstance(cpu, str) else cpu     # base/runner.py parse_cpu: cores -> millicores
         self.memory = memory
@@ -73,6 +75,9 @@ class TaskQueue:
         self.max_pending_tasks = max_pending_tasks
         self.name = name
         self.gpu_handler = gpu_handler or os.environ.get("B9_GPU_HANDLER", "identity")
+        # a user handler (b9gpu_handler.cuh): the sm_90a image (bytes or a path) that holds B9_HANDLER(gpu_handler, ...)
+        self.gpu_handler_image = gpu_handler_image or os.environ.get("B9_GPU_HANDLER_IMAGE") or None
+        self._handler_loaded = False
         self.device = device
         self.extra = kwargs
         self._queue = queue
@@ -83,6 +88,9 @@ class TaskQueue:
     def queue(self) -> DeviceQueue:
         if self._queue is None:
             self._queue = DeviceQueue(device=self.device)     # raises without a GPU: no CPU path
+        if self.gpu_handler_image is not None and not self._handler_loaded:
+            self._queue.load_handler(self.gpu_handler_image, self.gpu_handler)
+            self._handler_loaded = True
         if not self._policy_set:
             self._queue.set_retry_policy(self.retry_for, self.retries)
             if self.callback_url:

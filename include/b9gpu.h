@@ -64,6 +64,10 @@ enum b9_handler {
     B9_H_COUNT_
 };
 
+/* Ids from B9_H_USER_BASE on are user handlers: B9_H_USER_BASE + k is the k-th image b9_handler_load loaded into the
+ * context (ids belong to that context). */
+#define B9_H_USER_BASE 256
+
 /* ---- per-task status, reported in b9_results.status ---------------------------------------
  * COMPLETE/ERROR/RETRY are the runner's TaskStatus values (sdk/src/beta9/type.py TaskStatus,
  * set at sdk/src/beta9/runner/taskqueue.py:344-361). REJECTED means the reference would have
@@ -225,6 +229,22 @@ void        b9_ctx_destroy(b9_ctx *ctx);
 const char *b9_last_error(const b9_ctx *ctx);         /* ctx may be NULL for create failures     */
 const char *b9_handler_name(int handler);             /* "identity", "crc32", ...; NULL if unknown */
 int         b9_handler_id(const char *name);          /* inverse; B9_ENOSYS if unknown           */
+
+/* ---- user handlers: the user's own function in the handler slot --------------------------------------------------------
+ * A handler written against include/b9gpu_handler.cuh (a CUDA C++ header: a struct with a `call` template and a
+ * B9_HANDLER(name, Struct) line) and compiled to an sm_90a image is loaded with b9_handler_load. `image` is anything
+ * cudaLibraryLoadData accepts, an sm_90a cubin or a fatbin holding one, of `size` bytes; it is trusted code, as the
+ * process itself is. `name` is the B9_HANDLER name. The entry names carry the handler ABI version (B9_HANDLER_ABI_VERSION,
+ * kept with the drain's argument block): an image built against another version has no matching entry and the load fails
+ * with B9_EINVAL, naming the version. On success *handler_out = B9_H_USER_BASE + k, which b9_drain_launch, b9_drain and
+ * b9_endpoint_drain_launch take like a built-in id, with the same window, PEEK / ASYNC, claim, b9_running, B9_ENOSPC,
+ * callback and retry semantics; the tasks each rendering answers are the built-in handlers' (task-queue: SDK payloads,
+ * B9_TF_HTTP_BODY and B9_TF_TASK_MSG; endpoint: B9_TF_HTTP_BODY), B9_TF_PICKLE tasks are B9_ST_UNSUPPORTED, and
+ * B9_DRAIN_PICKLE_FULL with a user id is B9_EINVAL (nothing is consumed). An id this context did not return is B9_ENOSYS.
+ * A drain-side call. The images are unloaded by b9_ctx_destroy. b9_handler_name / b9_handler_id name built-in handlers
+ * only. Returns 0, or B9_EINVAL (NULL argument, a name that is not an identifier, an image that is not a cubin or fatbin
+ * within `size`, does not load, or lacks the entries), B9_EIO. Probe for it with dlsym. */
+int         b9_handler_load(b9_ctx *ctx, const void *image, uint64_t size, const char *name, int32_t *handler_out);
 
 /* page-locked host memory for callers (so that push/drain DMA straight from/to their buffers) */
 void       *b9_host_alloc(b9_ctx *ctx, uint64_t bytes);
