@@ -4,8 +4,8 @@
 //
 // The shape and the record rules are endpoint_drain_kernel's (endpoint_drain.cu): persistent warps of UD_WARPS-warp CTAs
 // take warp-tiles of UD_TILE consecutive slots from the control block's ticket, one task per lane. Each lane parses its
-// task (b9h::user_parse) and runs phase A (the handler with a counting sink); a ballot over the non-cancelled lanes gives
-// the record indices (count mode: plus the ready tasks before the tile, from tile_count_kernel run with UD_TILE), one
+// task (b9h::user_parse) and runs phase A (the handler with a counting sink, after binding the call to a declared
+// signature); a ballot over the non-cancelled lanes gives the record indices (count mode: plus the ready tasks before the tile, from tile_count_kernel run with UD_TILE), one
 // warp scan of the record lengths and one warp_reserve_bytes per tile, rounded up to 16 bytes as that kernel does, place
 // the bytes; each lane then writes its own record (phase B: a string result calls the handler again with a writing sink).
 // Under a retry policy (task-queue rendering) a status goes through retry_settle, which writes task_of for RETRY records.
@@ -35,7 +35,7 @@ __device__ __forceinline__ void user_drain(const DrainArgs& a) {
         const uint32_t slot = (uint32_t)((a.first_task + i) & a.slot_mask);
         const uint64_t h = in ? __ldg(a.hdr + slot) : 0ull;
         const bool live = in && !(hdr_flags(h) & 1u);
-        b9h::UserRec rec;
+        b9h::rec_t<H> rec;
         rec.status = ST_UNSUPPORTED; rec.has = 0; rec.vk = b9h::VK_UNSET; rec.out_len = 0; rec.src_off = 0; rec.src_len = 0; rec.value = 0;
         const uint8_t* p = a.payload;
         if (live) {
@@ -47,7 +47,7 @@ __device__ __forceinline__ void user_drain(const DrainArgs& a) {
                 const uint32_t w[4] = {id.x, id.y, id.z, id.w};
                 for (int b = 0; b < 16; ++b) idb[b] = (uint8_t)(w[b >> 2] >> (8 * (b & 3)));
             }
-            b9h::user_phase_a<H, R>(p, b9h::user_parse<R>(p, hdr_len(h), flags, idb), rec);
+            b9h::task_phase_a<H, R>(p, hdr_len(h), flags, idb, rec);
         }
 
         // ---- record index (ballot), bytes (scan) and ONE cursor add per warp-tile
@@ -65,7 +65,7 @@ __device__ __forceinline__ void user_drain(const DrainArgs& a) {
         if (R == b9h::TASK_QUEUE && a.retry_mask) status = retry_settle(a, j, i, status, rec.value);
         store_record_id(a.out, j, a.ids + slot);
         store_record(a.out, j, r.fits, ob, my, status, rec.has);
-        if (r.fits && rec.has && !b9h::user_phase_b<H, R>(p, rec, a.out.payload + ob))
+        if (r.fits && rec.has && !b9h::task_phase_b<H, R>(p, rec, a.out.payload + ob))
             store_record(a.out, j, true, 0, 0, (uint8_t)ST_UNSUPPORTED, 0);    // the handler's two passes disagreed
     }
 }

@@ -6,3 +6,6 @@ B9_HANDLER(echo_str, b9_examples::EchoStr)
 B9_HANDLER(crc32_str, b9_examples::Crc32Str)
 B9_HANDLER(word_count, b9_examples::WordCount)
 B9_HANDLER(prod, b9_examples::Prod)
+B9_HANDLER(greet, b9_examples::Greet)
+B9_HANDLER(join, b9_examples::Join)
+B9_HANDLER(field_sum, b9_examples::FieldSum)

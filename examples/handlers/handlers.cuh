@@ -114,4 +114,102 @@ struct Prod {
     }
 };
 
+// ---- handlers with a declared signature (B9H_SIGNATURE): `call` receives the bound call -------------------------------
+template <class Out> __device__ void put_str(const b9h::Arg& s, Out& out) {
+    b9h::Chars c = s.chars();
+    uint32_t cp;
+    while (c.next(cp)) out.cp(cp);
+}
+template <class Out> __device__ void put_ascii(const char* s, Out& out) { for (; *s; ++s) out.cp((uint8_t)*s); }
+
+// def greet(name, greeting="Hello", *, punct="!"): return greeting + ", " + name + punct
+// (str + a non-str raises TypeError)
+struct Greet {
+    B9H_SIGNATURE(B9H_POS_OR_KW("name"), B9H_POS_OR_KW_OPT("greeting"), B9H_KW_ONLY_OPT("punct"));
+    template <class Out> __device__ static int call(const b9h::Call& c, Out& out) {
+        for (int i = 0; i < 3; ++i)
+            if (c.has(i) && c[i].kind() != b9h::STR) return B9_EXC_TYPE_ERROR;
+        out.str_begin();
+        if (c.has(1)) put_str(c[1], out); else put_ascii("Hello", out);
+        put_ascii(", ", out);
+        put_str(c[0], out);
+        if (c.has(2)) put_str(c[2], out); else put_ascii("!", out);
+        out.str_end();
+        return 0;
+    }
+};
+
+// def join(sep, *parts):
+//     if type(sep) is not str or any(type(p) is not str for p in parts): raise TypeError
+//     return sep.join(parts)
+struct Join {
+    B9H_SIGNATURE(B9H_POS_OR_KW("sep"), B9H_VAR_POS("parts"));
+    template <class Out> __device__ static int call(const b9h::Call& c, Out& out) {
+        if (c[0].kind() != b9h::STR) return B9_EXC_TYPE_ERROR;
+        b9h::Items it = c.rest();
+        b9h::Arg x;
+        while (it.next(x)) if (x.kind() != b9h::STR) return B9_EXC_TYPE_ERROR;
+        out.str_begin();
+        it = c.rest();
+        for (bool first = true; it.next(x); first = false) {
+            if (!first) put_str(c[0], out);
+            put_str(x, out);
+        }
+        out.str_end();
+        return 0;
+    }
+};
+
+// def field_sum(rows, *, field):
+//     total = 0
+//     for row in rows:
+//         if type(row) is not dict: raise TypeError
+//         v = row[field]                                   (KeyError when the row has no such key)
+//         if type(v) not in (int, float, bool): raise TypeError
+//         total += v
+//     return total
+// A field that is not a str raises TypeError before the loop. ints add exactly while the sum fits in int64 (past it
+// the device declines: Python goes on with a big int); from the first float on, the sum is a float64 added left to right
+// in IEEE round-to-nearest. A str or dict `rows` iterates its characters / keys (TypeError, unless empty); other
+// non-iterables raise TypeError.
+struct FieldSum {
+    B9H_SIGNATURE(B9H_POS_OR_KW("rows"), B9H_KW_ONLY("field"));
+    template <class Out> __device__ static int call(const b9h::Call& c, Out& out) {
+        const b9h::Arg rows = c[0], field = c[1];
+        if (field.kind() != b9h::STR) return B9_EXC_TYPE_ERROR;
+        const int k = rows.kind();
+        if (k == b9h::STR || k == b9h::DICT) {
+            if (!rows.empty()) return B9_EXC_TYPE_ERROR;
+            out.integer(0);
+            return 0;
+        }
+        if (k != b9h::LIST) return B9_EXC_TYPE_ERROR;
+        long long si = 0; double sf = 0.0; bool fl = false;
+        b9h::Items it = rows.items();
+        b9h::Arg row, v;
+        while (it.next(row)) {
+            if (row.kind() != b9h::DICT) return B9_EXC_TYPE_ERROR;
+            if (!row.get(field, v)) return B9_EXC_KEY_ERROR;
+            const int kv = v.kind();
+            if (kv != b9h::INT && kv != b9h::FLOAT && kv != b9h::BOOL) return B9_EXC_TYPE_ERROR;
+            long long vi = 0; double vf = 0.0;
+            const int t = v.number(&vi, &vf);
+            if (t == B9H_DECLINE) return B9H_DECLINE;
+            if (t == b9h::FLOAT) {
+                if (!fl) { sf = (double)si; fl = true; }
+                sf = b9h::add_rn(sf, vf);
+            } else if (fl) {
+                sf = b9h::add_rn(sf, (double)vi);
+            } else {
+                const __int128 r = (__int128)si + vi;
+                if (r > (__int128)9223372036854775807ll || r < -(__int128)9223372036854775807ll - 1) return B9H_DECLINE;
+                si = (long long)r;
+            }
+        }
+        if (fl) out.real(sf);
+        else out.integer(si);
+        return 0;
+    }
+};
+
 }  // namespace b9_examples

@@ -27,4 +27,29 @@ def prod(xs, /):
     return p
 
 
-TWINS = {"echo_str": echo_str, "crc32_str": crc32_str, "word_count": word_count, "prod": prod}
+def greet(name, greeting="Hello", *, punct="!"):
+    return greeting + ", " + name + punct
+
+
+def join(sep, *parts):
+    if type(sep) is not str or any(type(p) is not str for p in parts):
+        raise TypeError("join joins strs")
+    return sep.join(parts)
+
+
+def field_sum(rows, *, field):
+    if type(field) is not str:
+        raise TypeError("field is a str")
+    total = 0
+    for row in rows:
+        if type(row) is not dict:
+            raise TypeError("field_sum sums the fields of dicts")
+        v = row[field]
+        if type(v) not in (int, float, bool):
+            raise TypeError("field_sum adds numbers")
+        total += v
+    return total
+
+
+TWINS = {"echo_str": echo_str, "crc32_str": crc32_str, "word_count": word_count, "prod": prod,
+         "greet": greet, "join": join, "field_sum": field_sum}

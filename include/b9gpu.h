@@ -95,7 +95,10 @@ enum b9_status {
  * The runner answers TaskStatus.Retry instead of Error when `type(e) is err` for an `err` in the stub's `retry_for`
  * (sdk/src/beta9/runner/taskqueue.py:352-393,407-408): an exact class match, so B9_EXC_VALUE_ERROR does not
  * cover binascii.Error. The classes the four handlers (oracle/pyoracle/handlers.py) can raise on CPython 3.12:   */
-#define B9_EXC_TYPE_ERROR       0x01u  /* any handler: not exactly one positional argument, or keyword arguments; vadd_f32 of a
+#define B9_EXC_TYPE_ERROR       0x01u  /* a handler without a declared signature: not exactly one positional argument, or
+                                          keyword arguments; one with a signature: any failure to bind the call to it (too
+                                          many positionals, a missing, unexpected or positional-only keyword, multiple
+                                          values for a parameter); vadd_f32 of a
                                           non-str; json_sum of a non-dict, of a "values" that is not iterable or holds a
                                           non-number (a dict "values" sums its str keys)                                     */
 #define B9_EXC_ATTRIBUTE_ERROR  0x02u  /* crc32 of a non-str (no .encode)                                                    */

@@ -2,7 +2,8 @@
 // cubin, and load it into a context with b9_handler_load.
 //
 // A handler is a struct with one function template. It receives args[0] of the call as the Python runner receives it
-// (b9h::Arg) and writes one result value into a sink (Out):
+// (b9h::Arg), or the whole call bound to a declared signature (b9h::Call, below), and writes one result value into a
+// sink (Out):
 //
 //     #include "b9gpu_handler.cuh"
 //     struct WordCount {                       // twin: def word_count(s, /): return len(s.split())
@@ -21,6 +22,24 @@
 //
 // The call rule is the built-in handlers': a positional-only one-parameter function. A call with anything but exactly one
 // positional argument and no keyword arguments is ERROR / TypeError before `call` runs.
+//
+// A handler may instead declare its Python signature; `call` then receives the bound call:
+//
+//     struct Greet {                           // twin: def greet(name, greeting="Hello", *, punct="!"): ...
+//         B9H_SIGNATURE(B9H_POS_OR_KW("name"), B9H_POS_OR_KW_OPT("greeting"), B9H_KW_ONLY_OPT("punct"));
+//         template <class Out> __device__ static int call(const b9h::Call& c, Out& out);   // c[i], c.has(i), c.rest()
+//     };
+//
+// Parameters (at most 8, in `def` order) are B9H_POS_ONLY, B9H_POS_OR_KW, B9H_VAR_POS (*args: c.rest() iterates the
+// surplus positionals) and B9H_KW_ONLY, each required or _OPT. An optional parameter not passed reads as absent
+// (c.has(i) == false) and the handler applies its default. Names are ASCII identifiers; `context` (the runner's
+// FunctionContext) is refused; static_asserts check both, and Python's parameter order. The call is bound as CPython binds
+// handler(*args, **kwargs): every failure (too many positionals, a missing required parameter, an unexpected keyword, a
+// positional-only name passed as a keyword, multiple values for one parameter) is ERROR / TypeError before `call` runs.
+// The arguments are the runner's: an SDK payload's args / kwargs as Go's struct decode kept them (kwargs objects that
+// Go would merge are UNSUPPORTED); an HTTP body's as SerializeHttpPayload makes them (a last "args" list is the
+// positionals, a last "kwargs" object alone is the kwargs, else the body's other top-level keys are); a record's own.
+// Keywords match by decoded code points, the last of duplicate keys deciding. Arg::get reads a dict by key the same way.
 //
 // `call` runs twice for a string result: once with a counting sink (status, length, falsiness), then, once the warp has
 // reserved the record's bytes, with a writing sink. It must therefore be deterministic: a second pass that writes another
@@ -60,6 +79,13 @@ __device__ __forceinline__ double mul_rn(double a, double b) {
     return __dmul_rn(a, b);
 #else
     return a * b;
+#endif
+}
+__device__ __forceinline__ double add_rn(double a, double b) {
+#ifdef __CUDA_ARCH__
+    return __dadd_rn(a, b);
+#else
+    return a + b;
 #endif
 }
 
@@ -103,6 +129,11 @@ public:
         return k;
     }
     __device__ Items items() const;
+    // DICT: the value of `key` as the runner's dict holds it (of duplicate keys the last one; keys compared by their
+    // decoded code points); false when the dict has no such key, or this is not a dict. `key` is a STR Arg (any other
+    // kind matches nothing) or a NUL-terminated UTF-8 string.
+    __device__ bool get(const Arg& key, Arg& out) const;
+    __device__ bool get(const char* key, Arg& out) const;
     // "", [], {}
     __device__ bool empty() const {
         const uint8_t c = p_[s_];
@@ -112,6 +143,7 @@ public:
     }
 
 private:
+    friend class Call;
     // number() without the range rule: *range = an int outside int64 (its kind is still INT)
     __device__ int num(long long* i, double* f, bool* range) const;
     const uint8_t* p_; uint32_t s_, e_; bool* unsure_;
@@ -133,6 +165,74 @@ struct Items {
 };
 
 __device__ inline Items Arg::items() const { Items it; it.p = p_; it.i = s_ + 1; it.e = e_; it.unsure = unsure_; return it; }
+
+// The members of a validated object whose body starts at i (just past its '{') and which ends before e, in text order:
+// key body [ks, ke) (between the quotes, still escaped), value [vs, ve)
+struct Members {
+    const uint8_t* p; uint32_t i, e;
+    __device__ bool next(uint32_t& ks, uint32_t& ke, uint32_t& vs, uint32_t& ve) {
+        while (b9::is_ws(p[i])) ++i;
+        if (p[i] == '}') return false;
+        if (p[i] == ',') { ++i; while (b9::is_ws(p[i])) ++i; }
+        uint32_t f = 0;
+        ks = i + 1;
+        i = (uint32_t)b9::scan_string(p, i, e, f);
+        ke = i - 1;
+        while (b9::is_ws(p[i]) || p[i] == ':') ++i;
+        vs = i;
+        i = (uint32_t)b9::skip_value(p, i, e, f);
+        ve = i;
+        return true;
+    }
+};
+
+// Does the decoded key body p[ks, ke) equal the UTF-8 bytes s[0, n)? Each decoded code point is encoded back to UTF-8
+// and compared, so a name or a C-string key is never decoded itself.
+__device__ inline bool key_eq(const uint8_t* p, uint32_t ks, uint32_t ke, const uint8_t* s, uint32_t n) {
+    uint32_t j = 0;
+    while (ks < ke) {
+        const uint32_t cp = b9::next_cp(p, ks, ke);
+        const uint32_t l = cp < 0x80 ? 1u : cp < 0x800 ? 2u : cp < 0x10000 ? 3u : 4u;
+        if (j + l > n) return false;
+        if (l == 1) { if (s[j] != cp) return false; }
+        else {
+            const uint8_t lead = l == 2 ? 0xC0 : l == 3 ? 0xE0 : 0xF0;
+            if (s[j] != (uint8_t)(lead | (cp >> (6 * (l - 1))))) return false;
+            for (uint32_t k = 1; k < l; ++k) if (s[j + k] != (uint8_t)(0x80 | ((cp >> (6 * (l - 1 - k))) & 0x3F))) return false;
+        }
+        j += l;
+    }
+    return j == n;
+}
+
+// ... or the decoded string body q[qs, qe)
+__device__ inline bool key_eq(const uint8_t* p, uint32_t ks, uint32_t ke, const uint8_t* q, uint32_t qs, uint32_t qe) {
+    while (ks < ke && qs < qe) if (b9::next_cp(p, ks, ke) != b9::next_cp(q, qs, qe)) return false;
+    return ks >= ke && qs >= qe;
+}
+
+__host__ __device__ constexpr uint32_t cstr_len(const char* s) { uint32_t n = 0; while (s[n]) ++n; return n; }
+
+__device__ inline bool Arg::get(const Arg& key, Arg& out) const {
+    if (p_[s_] != '{' || key.p_[key.s_] != '"') return false;
+    Members m{p_, s_ + 1, e_};
+    uint32_t ks, ke, vs, ve;
+    bool found = false;
+    while (m.next(ks, ke, vs, ve))
+        if (key_eq(p_, ks, ke, key.p_, key.s_ + 1, key.e_ - 1)) { out = Arg(p_, vs, ve, unsure_); found = true; }
+    return found;
+}
+
+__device__ inline bool Arg::get(const char* key, Arg& out) const {
+    if (p_[s_] != '{') return false;
+    const uint32_t n = cstr_len(key);
+    Members m{p_, s_ + 1, e_};
+    uint32_t ks, ke, vs, ve;
+    bool found = false;
+    while (m.next(ks, ke, vs, ve))
+        if (key_eq(p_, ks, ke, (const uint8_t*)key, n)) { out = Arg(p_, vs, ve, unsure_); found = true; }
+    return found;
+}
 
 __device__ inline int Arg::num(long long* i, double* f, bool* range) const {
     const uint8_t d = p_[s_];
@@ -242,6 +342,30 @@ template <int R> __device__ inline uint32_t scalar_write(uint8_t vk, long long v
     }
 }
 
+// What `call` returned (ret), whether it asked something the device cannot answer (unsure) and what it wrote (out) as
+// the record's status, has and length: the rules of user_phase_a below, for a handler with a signature (user_phase_a
+// keeps its own copy so that the one-Arg entries compile to the same code as before signatures existed).
+template <int R> __device__ inline bool phase_a_settle(int ret, bool unsure, const CountSink<R>& out, UserRec& rec) {
+    rec.status = b9::ST_UNSUPPORTED;
+    if (unsure) return false;
+    if (ret != 0) {
+        if (ret > 0 && ret <= (int)B9_EXC_ALL && !(ret & (ret - 1))) { rec.status = b9::ST_ERROR; rec.value = ret; }
+        return false;
+    }
+    if (out.vk == VK_UNSET || out.vk == VK_BAD || out.open) return false;
+    if (out.vk == VK_FLOAT && R == ENDPOINT && (((unsigned long long)out.v >> 52) & 0x7FFull) == 0x7FFull) return false;   // allow_nan=False
+    rec.status = b9::ST_OK;
+    rec.vk = out.vk; rec.value = out.v;
+    if (R == TASK_QUEUE) {                                        // `serialize_result(result) if result else None`
+        const bool falsy = out.vk == VK_NONE || ((out.vk == VK_BOOL || out.vk == VK_INT) && out.v == 0) ||
+                           (out.vk == VK_FLOAT && ((unsigned long long)out.v << 1) == 0) || (out.vk == VK_STR && out.cps == 0);
+        if (falsy) return false;
+    }
+    rec.has = 1;
+    rec.out_len = out.vk == VK_STR ? out.n : scalar_write<R>(out.vk, out.v, nullptr);
+    return true;
+}
+
 // Phase A: status, has and the record's length; `pr` is user_parse's
 template <class H, int R> __device__ inline void user_phase_a(const uint8_t* p, const b9::Parsed& pr, UserRec& rec) {
     rec.src_off = 0; rec.src_len = 0; rec.out_len = 0; rec.has = 0; rec.vk = VK_UNSET; rec.value = 0;
@@ -280,6 +404,218 @@ template <class H, int R> __device__ inline bool user_phase_b(const uint8_t* p, 
     WriteSink<R> out(o, rec.out_len);
     const int ret = H::call(arg, out);
     return ret == 0 && !unsure && out.ok && out.done && out.n == rec.out_len;
+}
+
+// ---- declared signatures ------------------------------------------------------------------------------------------
+// A handler that declares its Python signature with B9H_SIGNATURE receives the bound call (b9h::Call) instead of one Arg.
+enum ParamKind : uint8_t { P_POS_ONLY = 0, P_POS_OR_KW, P_VAR_POS, P_KW_ONLY };
+constexpr int MAX_PARAMS = 8;
+
+struct Param {
+    uint8_t kind; bool opt; const char* name;
+    __host__ __device__ constexpr Param() : kind(P_POS_ONLY), opt(false), name("") {}
+    __host__ __device__ constexpr Param(uint8_t k, bool o, const char* s) : kind(k), opt(o), name(s) {}
+};
+struct Sig {
+    int n; Param p[MAX_PARAMS];
+};
+template <class... Ps> __host__ __device__ constexpr Sig make_sig(Ps... ps) {
+    const Param a[] = {ps...};
+    Sig s{};
+    s.n = (int)sizeof...(ps);
+    for (int k = 0; k < s.n && k < MAX_PARAMS; ++k) s.p[k] = a[k];
+    return s;
+}
+
+// the compile-time checks B9H_SIGNATURE makes (each a static_assert of its own, so that the message names the rule)
+__host__ __device__ constexpr bool sig_names_ok(const Sig& s) {          // ASCII identifiers
+    for (int k = 0; k < s.n && k < MAX_PARAMS; ++k) {
+        const char* c = s.p[k].name;
+        if (!((c[0] >= 'A' && c[0] <= 'Z') || (c[0] >= 'a' && c[0] <= 'z') || c[0] == '_')) return false;
+        for (int j = 1; c[j]; ++j)
+            if (!((c[j] >= 'A' && c[j] <= 'Z') || (c[j] >= 'a' && c[j] <= 'z') || (c[j] >= '0' && c[j] <= '9') || c[j] == '_')) return false;
+    }
+    return true;
+}
+__host__ __device__ constexpr bool str_eq(const char* a, const char* b) {
+    int j = 0;
+    while (a[j] && a[j] == b[j]) ++j;
+    return a[j] == b[j];
+}
+__host__ __device__ constexpr bool sig_names_unique(const Sig& s) {
+    for (int k = 0; k < s.n && k < MAX_PARAMS; ++k)
+        for (int m = 0; m < k; ++m) if (str_eq(s.p[k].name, s.p[m].name)) return false;
+    return true;
+}
+__host__ __device__ constexpr bool sig_no_context(const Sig& s) {
+    for (int k = 0; k < s.n && k < MAX_PARAMS; ++k) if (str_eq(s.p[k].name, "context")) return false;
+    return true;
+}
+// Python's order: positional-only, positional-or-keyword, at most one *args, keyword-only; among the positional
+// parameters no required one after an optional one
+__host__ __device__ constexpr bool sig_order_ok(const Sig& s) {
+    bool opt_seen = false;
+    for (int k = 0; k < s.n && k < MAX_PARAMS; ++k) {
+        const Param& q = s.p[k];
+        if (q.kind > P_KW_ONLY) return false;
+        if (k && (q.kind < s.p[k - 1].kind || (q.kind == P_VAR_POS && s.p[k - 1].kind == P_VAR_POS))) return false;
+        if (q.kind <= P_POS_OR_KW) { if (opt_seen && !q.opt) return false; opt_seen = opt_seen || q.opt; }
+    }
+    return true;
+}
+
+#define B9H_POS_ONLY(n)      b9h::Param(b9h::P_POS_ONLY, false, n)
+#define B9H_POS_ONLY_OPT(n)  b9h::Param(b9h::P_POS_ONLY, true, n)
+#define B9H_POS_OR_KW(n)     b9h::Param(b9h::P_POS_OR_KW, false, n)
+#define B9H_POS_OR_KW_OPT(n) b9h::Param(b9h::P_POS_OR_KW, true, n)
+#define B9H_VAR_POS(n)       b9h::Param(b9h::P_VAR_POS, true, n)
+#define B9H_KW_ONLY(n)       b9h::Param(b9h::P_KW_ONLY, false, n)
+#define B9H_KW_ONLY_OPT(n)   b9h::Param(b9h::P_KW_ONLY, true, n)
+// Inside a handler struct: its Python signature, parameters in `def` order. Binding follows CPython's for
+// handler(*args, **kwargs); an optional parameter left unbound reads as absent and the handler applies its default.
+#define B9H_SIGNATURE(...)                                                                                                    \
+    __host__ __device__ static constexpr b9h::Sig b9h_signature() { return b9h::make_sig(__VA_ARGS__); }                      \
+    static_assert(b9h::make_sig(__VA_ARGS__).n <= b9h::MAX_PARAMS, "b9h: a signature has at most 8 parameters");             \
+    static_assert(b9h::sig_names_ok(b9h::make_sig(__VA_ARGS__)), "b9h: parameter names are ASCII identifiers");              \
+    static_assert(b9h::sig_names_unique(b9h::make_sig(__VA_ARGS__)), "b9h: duplicate parameter name");                       \
+    static_assert(b9h::sig_no_context(b9h::make_sig(__VA_ARGS__)),                                                           \
+                  "b9h: `context` is the runner's FunctionContext, which the device cannot bind");                           \
+    static_assert(b9h::sig_order_ok(b9h::make_sig(__VA_ARGS__)),                                                             \
+                  "b9h: parameters go positional-only, positional-or-keyword, *args, keyword-only, positional defaults last")
+
+template <class...> struct void_t_ { typedef void type; };
+template <class H, class = void> struct has_signature { static constexpr bool value = false; };
+template <class H> struct has_signature<H, typename void_t_<decltype(H::b9h_signature())>::type> { static constexpr bool value = true; };
+
+// Where a call's arguments are: the positional list p[a_off, a_off + a_len) (a_len 0: none) and the kwargs object
+// p[k_off, k_off + k_len) (k_len 0: none). k_skip_args: the object is an HTTP body's top level, whose "args" members
+// were taken as the positionals (SerializeHttpPayload deletes that key).
+struct CallSrc { uint32_t a_off, a_len, k_off, k_len; uint8_t k_skip_args; };
+
+// The bound call, by parameter index in the signature: c[i] is the bound value, c.has(i) whether there is one (an
+// optional parameter not passed reads as absent), c.rest() the positionals *args collected.
+class Call {
+public:
+    __device__ Arg operator[](int i) const { return Arg(p_, s_[i], e_[i], unsure_); }
+    __device__ bool has(int i) const { return e_[i] != 0; }
+    __device__ Items rest() const { Items it; it.p = rp_; it.i = ri_; it.e = re_; it.unsure = unsure_; return it; }
+
+    // CPython's binding of handler(*args, **kwargs) to H's signature; false where it raises TypeError
+    template <class H> __device__ bool bind(const uint8_t* p, const CallSrc& src, bool* unsure);
+
+private:
+    const uint8_t* p_; bool* unsure_;
+    uint32_t s_[MAX_PARAMS], e_[MAX_PARAMS];
+    const uint8_t* rp_; uint32_t ri_, re_;
+};
+
+template <class H> __device__ inline bool Call::bind(const uint8_t* p, const CallSrc& src, bool* unsure) {
+    constexpr Sig S = H::b9h_signature();
+    p_ = p; unsure_ = unsure;
+#pragma unroll
+    for (int k = 0; k < MAX_PARAMS; ++k) { s_[k] = 0; e_[k] = 0; }
+    int npos = 0; bool var = false;
+#pragma unroll
+    for (int k = 0; k < S.n; ++k) { npos += S.p[k].kind <= P_POS_OR_KW; var = var || S.p[k].kind == P_VAR_POS; }
+    // positionals: the first npos to the positional parameters, the others to *args
+    int bound = 0;
+    rp_ = (const uint8_t*)"]"; ri_ = 0; re_ = 1;
+    if (src.a_len) {
+        Items it; it.p = p; it.i = src.a_off + 1; it.e = src.a_off + src.a_len; it.unsure = unsure;
+        Arg x;
+#pragma unroll
+        for (int k = 0; k < MAX_PARAMS; ++k) {
+            if (k >= npos || !it.next(x)) break;
+            s_[k] = x.s_; e_[k] = x.e_; ++bound;
+        }
+        rp_ = p; ri_ = it.i; re_ = it.e;
+        if (!var && bound == npos && it.next(x)) return false;                    // too many positional arguments
+    }
+    // keywords: by decoded name, the last member of a name deciding
+    if (src.k_len) {
+        Members m{p, src.k_off + 1, src.k_off + src.k_len};
+        uint32_t ks, ke, vs, ve;
+        while (m.next(ks, ke, vs, ve)) {
+            if (src.k_skip_args && b9::match_exact_key(p, ks, ke) == 1) continue;
+            bool hit = false;
+#pragma unroll
+            for (int k = 0; k < S.n; ++k) {
+                if (S.p[k].kind == P_VAR_POS || hit) continue;
+                if (!key_eq(p, ks, ke, (const uint8_t*)S.p[k].name, cstr_len(S.p[k].name))) continue;
+                if (S.p[k].kind == P_POS_ONLY || k < bound) return false;         // positional-only by keyword; multiple values
+                s_[k] = vs; e_[k] = ve; hit = true;
+            }
+            if (!hit) return false;                                               // unexpected keyword argument
+        }
+    }
+#pragma unroll
+    for (int k = 0; k < S.n; ++k)
+        if (S.p[k].kind != P_VAR_POS && !S.p[k].opt && !e_[k]) return false;     // missing required argument
+    return true;
+}
+
+// Where rendering R's task p[0, n) with slot flags `flags` has its arguments (pr: user_parse's, ST_OK). flags 0: the SDK
+// payload's args / kwargs as Go's struct decode kept them; B9_TF_TASK_MSG: the record's own; B9_TF_HTTP_BODY:
+// SerializeHttpPayload -- a last "args" that is a list is the positionals, a last "kwargs" that is an object alone is
+// the kwargs, otherwise every other top-level key of the body is a keyword argument.
+__device__ inline CallSrc call_src(const uint8_t* p, uint32_t n, uint32_t flags, const b9::Parsed& pr) {
+    CallSrc c; c.a_off = pr.args_off; c.a_len = pr.args_len; c.k_off = pr.kw_off; c.k_len = pr.kw_len; c.k_skip_args = 0;
+    if (flags == B9_TF_HTTP_BODY && !pr.kw_len) {
+        uint32_t i = 0;
+        while (i < n && b9::is_ws(p[i])) ++i;
+        if (i < n && p[i] == '{') {                                                // (else an empty or null body: no keys)
+            uint32_t f = 0;
+            c.k_off = i; c.k_len = (uint32_t)b9::skip_value(p, i, n, f) - i; c.k_skip_args = pr.args_len != 0;
+        }
+    }
+    return c;
+}
+
+struct CallRec : UserRec {
+    CallSrc src;                 // pass 2 of a string result binds the call again from here
+};
+
+// Phase A of a handler with a signature. A task-queue SDK payload whose "kwargs" came more than once as objects (Go
+// merges those maps) is UNSUPPORTED.
+template <class H, int R> __device__ inline void call_phase_a(const uint8_t* p, uint32_t n, uint32_t flags, const uint8_t* id, CallRec& rec) {
+    const b9::Parsed pr = user_parse<R>(p, n, flags, id);
+    rec.src_off = 0; rec.src_len = 0; rec.out_len = 0; rec.has = 0; rec.vk = VK_UNSET; rec.value = 0;
+    if (pr.status != b9::ST_OK) { rec.status = pr.status; return; }
+    if (flags == 0 && pr.kw_merged) { rec.status = b9::ST_UNSUPPORTED; return; }
+    rec.src = call_src(p, n, flags, pr);
+    bool unsure = false;
+    Call c;
+    if (!c.bind<H>(p, rec.src, &unsure)) { rec.status = b9::ST_ERROR; rec.value = B9_EXC_TYPE_ERROR; return; }
+    CountSink<R> out;
+    const int ret = H::call(c, out);
+    phase_a_settle<R>(ret, unsure, out, rec);
+}
+
+template <class H, int R> __device__ inline bool call_phase_b(const uint8_t* p, const CallRec& rec, uint8_t* o) {
+    if (rec.vk != VK_STR) { scalar_write<R>(rec.vk, rec.value, o); return true; }
+    bool unsure = false;
+    Call c;
+    if (!c.bind<H>(p, rec.src, &unsure)) return false;
+    WriteSink<R> out(o, rec.out_len);
+    const int ret = H::call(c, out);
+    return ret == 0 && !unsure && out.ok && out.done && out.n == rec.out_len;
+}
+
+// What the kernel runs for handler H: the one-Arg phases, or, for a handler with a signature, the bound call's
+template <bool Signature> struct RecSel { typedef UserRec type; };
+template <> struct RecSel<true> { typedef CallRec type; };
+template <class H> using rec_t = typename RecSel<has_signature<H>::value>::type;
+template <class H, int R> __device__ __forceinline__ void task_phase_a(const uint8_t* p, uint32_t n, uint32_t flags, const uint8_t* id, UserRec& rec) {
+    user_phase_a<H, R>(p, user_parse<R>(p, n, flags, id), rec);
+}
+template <class H, int R> __device__ __forceinline__ bool task_phase_b(const uint8_t* p, const UserRec& rec, uint8_t* o) {
+    return user_phase_b<H, R>(p, rec, o);
+}
+template <class H, int R> __device__ __forceinline__ void task_phase_a(const uint8_t* p, uint32_t n, uint32_t flags, const uint8_t* id, CallRec& rec) {
+    call_phase_a<H, R>(p, n, flags, id, rec);
+}
+template <class H, int R> __device__ __forceinline__ bool task_phase_b(const uint8_t* p, const CallRec& rec, uint8_t* o) {
+    return call_phase_b<H, R>(p, rec, o);
 }
 
 }  // namespace b9h
