@@ -15,7 +15,7 @@ PKG = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(PKG)
 CSRC = os.path.join(PKG, "csrc")
 SO = os.path.join(PKG, "libb9gpu.so")
-SOURCES = ["b9gpu.cu", "wire_full.cu", "function_drain.cu", "endpoint_drain.cu", "callback_sign.cu", "callback_runners.cu"]   # (all but b9gpu.cu: kernels in modules of their own)
+SOURCES = ["b9gpu.cu", "wire_full.cu", "endpoint_drain.cu", "drain_passes.cu"]   # (all but b9gpu.cu: kernels in modules of their own)
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 
 FLAGS = [

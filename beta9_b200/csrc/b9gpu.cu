@@ -41,22 +41,25 @@
 // wire_encode_kernel<true> for b9_wire_encode_full, launched from its own translation unit (wire_full.cu says why);
 // args: a WireArgs, env: the device copy of the WireEnv
 cudaError_t launch_wire_encode_full(const void* args, size_t args_size, const void* env, uint32_t grid, cudaStream_t s);
-// pickle_pass_kernel for B9_DRAIN_PICKLE_FULL, from function_drain.cu; args: the drain's DrainArgs
-cudaError_t launch_pickle_pass(const void* args, size_t args_size, int handler, int sm_count, cudaStream_t s);
-// callback_sign_kernel for b9_set_callback_policy, from callback_sign.cu; args: the drain's DrainArgs (tile_tasks as
-// launch_drain3 chose it), mid: the key's midstates (callback_midstates), keyed = 0: kinds only
+// the passes that run after the drain kernel, from drain_passes.cu; args: the drain's DrainArgs (tile_tasks as the drain
+// kernel used it). The callback sign pass (b9_set_callback_policy): mid: the key's midstates (callback_midstates), keyed = 0:
+// kinds only.
 void callback_midstates(const uint8_t* key, uint32_t key_len, uint32_t mid[16]);
 cudaError_t launch_callback_sign(const void* args, size_t args_size, const uint32_t mid[16], int keyed, int64_t ts,
                                  uint8_t* kind, uint8_t* digest, int sm_count, cudaStream_t s);
+// The runners' callback passes (b9_set_callback_runners); drain_passes.cu defines the same struct. out: kind, digest,
+// body_off, body_len, url_off, url_len.
+struct CallbackPassArgs { const uint32_t* mid; int keyed; int64_t ts; void* out[6]; };
+// the function pass for B9_DRAIN_PICKLE_FULL: cb == nullptr, the pickle pass; otherwise the function runner's callback
+// pass, which does the pickle pass's work behind the sign pass
+cudaError_t launch_function_pass(const void* args, size_t args_size, int handler, const CallbackPassArgs* cb, int sm_count, cudaStream_t s);
+// the endpoint runner's callback pass, behind endpoint_drain_kernel
+cudaError_t launch_endpoint_callbacks(const void* args, size_t args_size, const CallbackPassArgs& cb, cudaStream_t s);
 // endpoint_drain_kernel for b9_endpoint_drain_launch, from endpoint_drain.cu; args: the drain's DrainArgs, with tile_tasks
 // = ENDPOINT_TILE_TASKS and n_tiles set for it
 cudaError_t launch_endpoint_drain(const void* args, size_t args_size, int handler, int sm_count, cudaStream_t s);
 constexpr uint32_t ENDPOINT_TILE_TASKS = 32;   // endpoint_drain.cu's EP_TILE (the launcher refuses any other)
 constexpr int USER_DRAIN_WARPS = 4;            // user_drain.cuh's UD_WARPS (its tiles are ENDPOINT_TILE_TASKS slots too)
-// the function runner's callback pass (in place of the pickle pass, behind callback_sign_kernel) or the endpoint runner's
-// (behind endpoint_drain_kernel), from callback_runners.cu; out: kind, digest, body_off, body_len, url_off, url_len
-cudaError_t launch_callback_runner(int endpoint, const void* args, size_t args_size, int handler, const uint32_t mid[16], int keyed,
-                                   int64_t ts, void* const out[6], int sm_count, cudaStream_t s);
 
 using namespace b9;
 
@@ -1383,6 +1386,11 @@ static int64_t drain_launch_common(b9_ctx* c, int handler, uint32_t max_tasks, i
     // by whatever comes next (end_drain_span), the control block is read back by finish_launch
     const bool overlap = c->last_op_drain;
     c->last_op_drain = false;
+    // a launch that failed leaves the control block and the stream's order unknown to the host
+    auto launch_failed = [c](const char* what, cudaError_t e) {
+        c->last_op_drain = false; c->ctl_dirty = true;
+        return fail(B9_EIO, "%s launch failed: %s", what, cudaGetErrorString(e));
+    };
     cudaError_t le;
     uint32_t tt = 0;
     if (endpoint || user) {
@@ -1402,10 +1410,7 @@ static int64_t drain_launch_common(b9_ctx* c, int handler, uint32_t max_tasks, i
             void* args[] = {&a};
             le = cudaLaunchKernel((const void*)(endpoint ? user->ep : user->tq), dim3(ctas), dim3(USER_DRAIN_WARPS * 32), args, 0, s);
         }
-        if (le != cudaSuccess) {
-            c->ctl_dirty = true;
-            return fail(B9_EIO, "%s drain kernel launch failed: %s", user ? "user handler" : "endpoint", cudaGetErrorString(le));
-        }
+        if (le != cudaSuccess) return launch_failed(user ? "user handler drain kernel" : "endpoint drain kernel", le);
         c->last_op_drain = true;
         c->burst_open = true;
         if (!c->res.cb) end_drain_span(c);                                  // (with the runner's callback pass: behind that)
@@ -1416,7 +1421,7 @@ static int64_t drain_launch_common(b9_ctx* c, int handler, uint32_t max_tasks, i
     default:            le = launch_drain3<3>(a, in_bytes / n, win_max_len, c->stage_bytes_override, c->sm_count, overlap, s, &grid, &tt); break;
     }
     if (!endpoint && !user) {
-        if (le != cudaSuccess) { c->ctl_dirty = true; return fail(B9_EIO, "drain kernel launch failed: %s", cudaGetErrorString(le)); }
+        if (le != cudaSuccess) return launch_failed("drain kernel", le);
         c->last_op_drain = true;
         c->burst_open = true;
     }
@@ -1427,27 +1432,28 @@ static int64_t drain_launch_common(b9_ctx* c, int handler, uint32_t max_tasks, i
     // the function runner's callbacks (b9_set_callback_runners): its pass does the pickle pass's work and runs behind the
     // sign pass, whose B9_CB_HOST it overwrites for the pickle slots
     const bool function_runner = pickle_pass && c->res.cb && (c->cb_runners & B9_CB_RUNNER_FUNCTION);
-    void* const rq_out[6] = {c->d_cb_kind, c->d_cb_digest, c->d_cb_body_off, c->d_cb_body_len, c->d_cb_url_off, c->d_cb_url_len};
+    const CallbackPassArgs cb = {c->cb_mid, c->res.cb_keyed ? 1 : 0, c->res.cb_ts,
+                                 {c->d_cb_kind, c->d_cb_digest, c->d_cb_body_off, c->d_cb_body_len, c->d_cb_url_off, c->d_cb_url_len}};
     if (pickle_pass && !function_runner) {
         a.tile_tasks = tt;
-        le = launch_pickle_pass(&a, sizeof a, handler, c->sm_count, s);
-        if (le != cudaSuccess) { c->last_op_drain = false; c->ctl_dirty = true; return fail(B9_EIO, "pickle pass launch failed: %s", cudaGetErrorString(le)); }
+        le = launch_function_pass(&a, sizeof a, handler, nullptr, c->sm_count, s);
+        if (le != cudaSuccess) return launch_failed("pickle pass", le);
     }
-    // under a callback policy: every record's callback kind and signature (callback_sign.cu), behind the records' last
+    // under a callback policy: every record's callback kind and signature (drain_passes.cu), behind the records' last
     // writer (drain3_kernel or the pickle pass). Like the pickle pass it is never a programmatic dependent, the next drain
     // kernel waits for it in full, and the timed span ends behind it. It reads this launch's control block and count
-    // prefixes, which nothing rewrites before the next launch. The runners' passes (callback_runners.cu) follow the same rules.
+    // prefixes, which nothing rewrites before the next launch. The runners' passes follow the same rules.
     if (c->res.cb && endpoint) {
-        le = launch_callback_runner(1, &a, sizeof a, handler, c->cb_mid, c->res.cb_keyed ? 1 : 0, c->res.cb_ts, rq_out, c->sm_count, s);
-        if (le != cudaSuccess) { c->last_op_drain = false; c->ctl_dirty = true; return fail(B9_EIO, "endpoint callback pass launch failed: %s", cudaGetErrorString(le)); }
+        le = launch_endpoint_callbacks(&a, sizeof a, cb, s);
+        if (le != cudaSuccess) return launch_failed("endpoint callback pass", le);
         c->res.cb_requests = true;
     } else if (c->res.cb) {
         a.tile_tasks = tt;
-        le = launch_callback_sign(&a, sizeof a, c->cb_mid, c->res.cb_keyed ? 1 : 0, c->res.cb_ts, c->d_cb_kind, c->d_cb_digest, c->sm_count, s);
-        if (le != cudaSuccess) { c->last_op_drain = false; c->ctl_dirty = true; return fail(B9_EIO, "callback sign pass launch failed: %s", cudaGetErrorString(le)); }
+        le = launch_callback_sign(&a, sizeof a, c->cb_mid, cb.keyed, c->res.cb_ts, c->d_cb_kind, c->d_cb_digest, c->sm_count, s);
+        if (le != cudaSuccess) return launch_failed("callback sign pass", le);
         if (function_runner) {
-            le = launch_callback_runner(0, &a, sizeof a, handler, c->cb_mid, c->res.cb_keyed ? 1 : 0, c->res.cb_ts, rq_out, c->sm_count, s);
-            if (le != cudaSuccess) { c->last_op_drain = false; c->ctl_dirty = true; return fail(B9_EIO, "function callback pass launch failed: %s", cudaGetErrorString(le)); }
+            le = launch_function_pass(&a, sizeof a, handler, &cb, c->sm_count, s);
+            if (le != cudaSuccess) return launch_failed("function callback pass", le);
             c->res.cb_requests = true;
         }
     }

@@ -16,6 +16,7 @@
 // compressed once per key (cb_midstates), so a record costs its inner blocks plus one outer block.
 #pragma once
 #include <stdint.h>
+#include "json_device.cuh"
 
 namespace b9 {
 
@@ -232,7 +233,6 @@ __host__ __device__ __forceinline__ bool cb_nonfinite(const uint8_t* r, uint32_t
     return eq("NaN", 3) || eq("Infinity", 8) || eq("-Infinity", 9);
 }
 
-#ifdef B9_CALLBACK_KWARGS      // (needs json_device.cuh: the device build and the host shim define it)
 // ---- does the handler's kwargs hold a "callback_url" key? ----------------------------------------------------------
 // The runner reads override_callback_url = kwargs.get("callback_url"). Only the decoded key matters, as Python sees it
 // after Go's re-encoding: Go's unquote (next_cp), compared with the 12 ASCII bytes.
@@ -307,57 +307,5 @@ __device__ inline bool cb_kwargs_have_callback_url(const uint8_t* __restrict__ p
     }
     return mode == 1 ? (kw_dict ? found : top) : found;
 }
-#endif
 
 }  // namespace b9
-
-#if defined(__CUDACC__) && !defined(B9_CALLBACK_NO_SIGN_KERNEL)   // (callback_runners.cu uses the signing code only)
-namespace b9 {
-// One pass over a drain's records, right after the drain kernel (and the pickle pass). Thread per window task: its record
-// index is the task's in a dense window, else the count pre-pass's tile prefix plus the tile's ready slots before it
-// (as the pickle pass finds it). kind[j] is the record's b9_callback_kind; digest[j] its raw HMAC for a B9_CB_POST under a
-// key, otherwise zero. `empty` is the digest of {"data": {}}, the same for every such record of the drain.
-__global__ void __launch_bounds__(128) callback_sign_kernel(DrainArgs a, CbSign sg, uint32_t keyed, uint4 empty0, uint4 empty1,
-                                                            uint8_t* __restrict__ kind, uint4* __restrict__ digest) {
-    const DrainCtl* ctl = a.out.ctl;
-    if (ctl->overflow) return;                                     // B9_ENOSPC: no records to sign
-    for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < a.n_tasks; t += gridDim.x * blockDim.x) {
-        const uint32_t slot = (uint32_t)((a.first_task + t) & a.slot_mask);
-        const uint64_t h = a.hdr[slot];
-        const uint32_t flags = hdr_flags(h);
-        uint32_t j = t;
-        if (a.count_mode) {
-            if (flags & 1u) continue;                              // cancelled: no record
-            const uint32_t tile = t / a.tile_tasks;
-            j = tile_ready_before(a, tile, a.tile_tasks);
-            for (uint32_t q = tile * a.tile_tasks; q < t; ++q) j += (hdr_flags(a.hdr[(uint32_t)((a.first_task + q) & a.slot_mask)]) & 1u) ? 0u : 1u;
-        }
-        const uint8_t st = a.out.status[j];
-        uint8_t k;
-        bool sign_r = false;
-        if (flags & B9_TF_PICKLE_BIT) k = CB_HOST;
-        else if (st == ST_UNSUPPORTED) k = CB_HOST;
-        else if (st == ST_OK) {
-            if (!a.out.has[j]) k = CB_POST;
-            else if (cb_nonfinite(a.out.payload + a.out.off[j], a.out.len[j])) k = CB_UNSENDABLE;
-            else { k = CB_POST; sign_r = true; }
-        } else if (st == ST_ERROR) {
-            const int mode = (flags & B9_TF_TASK_MSG_BIT) ? 2 : (flags & B9_TF_HTTP_BODY_BIT) ? 1 : 0;
-            k = cb_kwargs_have_callback_url(a.payload + a.off[slot], hdr_len(h), mode) ? CB_HOST : CB_POST;
-        } else k = CB_NONE;                                        // REJECTED, RETRY, RETRY_LIMIT
-        kind[j] = k;
-        uint4 d0 = make_uint4(0, 0, 0, 0), d1 = d0;
-        if (keyed && k == CB_POST) {
-            if (sign_r) {
-                uint32_t o[8];
-                cb_sign_record(sg, a.out.payload + a.out.off[j], a.out.len[j], o);
-                // raw digest bytes in order: each big-endian word byte-swapped into the little-endian store
-                d0 = make_uint4(__byte_perm(o[0], 0, 0x0123), __byte_perm(o[1], 0, 0x0123), __byte_perm(o[2], 0, 0x0123), __byte_perm(o[3], 0, 0x0123));
-                d1 = make_uint4(__byte_perm(o[4], 0, 0x0123), __byte_perm(o[5], 0, 0x0123), __byte_perm(o[6], 0, 0x0123), __byte_perm(o[7], 0, 0x0123));
-            } else { d0 = empty0; d1 = empty1; }
-        }
-        digest[2 * (size_t)j] = d0; digest[2 * (size_t)j + 1] = d1;
-    }
-}
-}  // namespace b9
-#endif

@@ -167,6 +167,16 @@ constexpr uint32_t TC_SLOTS = 256;             // slots per tile_count_kernel bl
 __device__ __forceinline__ uint32_t tile_ready_before(const DrainArgs& a, unsigned long long tile, uint32_t T) {
     return __ldg(a.tile_base + tile) + __ldg(a.block_base + (uint32_t)((tile * T) / TC_SLOTS));
 }
+// the record index of window task t, which is not cancelled, for the passes that run after the drain kernel: t in a dense
+// window; in count mode the ready tasks before its warp-tile plus the ready slots before it in the tile (a.tile_tasks as
+// the drain kernel used it)
+__device__ __forceinline__ uint32_t window_record(const DrainArgs& a, uint32_t t) {
+    if (!a.count_mode) return t;
+    const uint32_t tile = t / a.tile_tasks;
+    uint32_t j = tile_ready_before(a, tile, a.tile_tasks);
+    for (uint32_t q = tile * a.tile_tasks; q < t; ++q) j += (hdr_flags(a.hdr[(uint32_t)((a.first_task + q) & a.slot_mask)]) & 1u) ? 0u : 1u;
+    return j;
+}
 
 // warp-cooperative byte copy global -> global (arbitrary alignment on both sides).
 // 16-byte stores on the destination, 4-byte loads + funnel shift on the source.

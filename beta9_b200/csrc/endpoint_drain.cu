@@ -3,7 +3,7 @@
 //
 // Why not in b9gpu.cu: NVVM decides inlining for a whole module, so a new kernel that calls the JSON and sum helpers
 // would change how the drain kernels compile (wire_full.cu measured that). The device headers are included inside an
-// anonymous namespace, as function_drain.cu does: their out-of-line __device__ functions get host-side definitions in
+// anonymous namespace, as wire_full.cu does: their out-of-line __device__ functions get host-side definitions in
 // every translation unit that includes them, which would clash with b9gpu.cu's at link time.
 //
 // Shape: persistent warps take warp-tiles of EP_TILE consecutive slots from the control block's ticket, one task per

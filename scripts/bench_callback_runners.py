@@ -8,7 +8,7 @@ drained with B9_DRAIN_PEEK under a callback policy (a 32-byte key), R times with
 alternated on the same ctx:
   - drain_ms_plain / drain_ms_runner: the median CUDA-event span around the launch's kernels (b9_stats.last_drain_kernel_ms);
     without the bit the pickle records are B9_CB_HOST and an endpoint launch runs no callback pass;
-  - runner_kernel_ms: the runner's own pass (function_callback_kernel / endpoint_callback_kernel), from torch.profiler's
+  - runner_kernel_ms: the runner's own pass (function_pass_kernel<3, true> / endpoint_callback_kernel), from torch.profiler's
     CUDA activity over R launches (median);
   - d_bytes: the callback JSON bytes the pass wrote; kinds: the b9_callback_kind counts.
 Prints one JSON line with the card's name and power limit read in the same run. Writes nothing.
@@ -51,7 +51,7 @@ def main() -> None:
     info = card()
     if a.runner == "function":
         b = synth.function_docs_batch(25_000)
-        handler, flags, name = "json_sum", L.TF_PICKLE, "function_callback_kernel"
+        handler, flags, name = "json_sum", L.TF_PICKLE, "function_pass_kernel"   # (only the runner's launches are profiled)
         launch_kw = dict(full_pickle=True)
     else:
         b = synth.strings_batch(1 << 20, 256)

@@ -7,8 +7,6 @@
 #define __host__
 #define __forceinline__ inline
 #define __constant__ static const
-#define B9_CALLBACK_KWARGS 1
-#include "../../beta9_b200/csrc/json_device.cuh"
 #include "../../beta9_b200/csrc/callback_sign.cuh"
 
 static void words_to_bytes(const uint32_t w[8], uint8_t out[32]) {
