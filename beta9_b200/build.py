@@ -96,6 +96,16 @@ def build_examples(force: bool = False) -> str:
     return compile_handlers(EXAMPLE_HANDLERS, EXAMPLE_CUBIN, force=force)
 
 
+TEST_HANDLERS = os.path.join(ROOT, "tests", "handlers", "contract.cu")
+TEST_CUBIN = os.path.join(ROOT, "tests", "handlers", "contract.cubin")   # build product (git-ignored)
+
+
+def build_test_handlers(force: bool = False) -> str:
+    """The test-only contract handlers (tests/handlers) as tests/handlers/contract.cubin, so that the GPU tests need no
+    nvcc."""
+    return compile_handlers(TEST_HANDLERS, TEST_CUBIN, force=force)
+
+
 def build_variant(name: str, defines: List[str]) -> str:
     """An alternative build for A/B timing on one box: ab_builds/<name>.so compiled with extra -D switches
     (selected at run time with B9GPU_LIB=...). ab_builds/ is git-ignored."""
@@ -116,3 +126,4 @@ if __name__ == "__main__":
         sys.exit(0)
     print(build(force="--force" in sys.argv, verbose_ptxas="--ptxas-v" in sys.argv))
     print(build_examples(force="--force" in sys.argv))
+    print(build_test_handlers(force="--force" in sys.argv))

@@ -167,7 +167,9 @@ struct Items {
 __device__ inline Items Arg::items() const { Items it; it.p = p_; it.i = s_ + 1; it.e = e_; it.unsure = unsure_; return it; }
 
 // The members of a validated object whose body starts at i (just past its '{') and which ends before e, in text order:
-// key body [ks, ke) (between the quotes, still escaped), value [vs, ve)
+// key body [ks, ke) (between the quotes, still escaped), value [vs, ve). An internal helper of Arg::get and Call::bind,
+// not part of the handler contract: it walks the text, duplicates included, while the runner's dict holds Go's sorted,
+// de-duplicated keys; a handler reads a dict through Arg::get.
 struct Members {
     const uint8_t* p; uint32_t i, e;
     __device__ bool next(uint32_t& ks, uint32_t& ke, uint32_t& vs, uint32_t& ve) {

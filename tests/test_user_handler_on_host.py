@@ -5,6 +5,7 @@ twins (examples/handlers/handlers.py) run through the oracle's loops: the task-q
 bodies, the runner's half over TaskMessage records, and the endpoint request. Statuses, has_result, record bytes and the
 exception class of every ERROR must agree; an UNSUPPORTED must carry one of the documented reasons (`may_decline`).
 echo_str and crc32_str must also equal the built-in identity and crc32 host builds wherever the argument is a str."""
+import binascii
 import ctypes as C
 import json
 import os
@@ -34,7 +35,7 @@ GXX = os.environ.get("CXX", "g++")
 NAMES = ["echo_str", "crc32_str", "word_count", "prod"]
 COMPLETE, ERROR, REJECTED, UNSUPPORTED = 0, 1, 3, 4
 TF_HTTP_BODY, TF_TASK_MSG = 0x02, 0x08
-EXC = {TypeError: 0x01, AttributeError: 0x02, UnicodeEncodeError: 0x04, KeyError: 0x08, ValueError: 0x10}
+EXC = {TypeError: 0x01, AttributeError: 0x02, UnicodeEncodeError: 0x04, KeyError: 0x08, ValueError: 0x10, binascii.Error: 0x20}
 TQ, ENDPOINT = 0, 1
 
 
