@@ -98,11 +98,14 @@ def build_examples(force: bool = False) -> str:
 
 TEST_HANDLERS = os.path.join(ROOT, "tests", "handlers", "contract.cu")
 TEST_CUBIN = os.path.join(ROOT, "tests", "handlers", "contract.cubin")   # build product (git-ignored)
+CONTAINER_HANDLERS = os.path.join(ROOT, "tests", "handlers", "containers.cu")
+CONTAINER_CUBIN = os.path.join(ROOT, "tests", "handlers", "containers.cubin")   # build product (git-ignored)
 
 
 def build_test_handlers(force: bool = False) -> str:
-    """The test-only contract handlers (tests/handlers) as tests/handlers/contract.cubin, so that the GPU tests need no
-    nvcc."""
+    """The test-only handlers (tests/handlers) as tests/handlers/contract.cubin and containers.cubin, so that the GPU
+    tests need no nvcc. Returns the first."""
+    compile_handlers(CONTAINER_HANDLERS, CONTAINER_CUBIN, force=force)
     return compile_handlers(TEST_HANDLERS, TEST_CUBIN, force=force)
 
 

@@ -9,3 +9,7 @@ B9_HANDLER(prod, b9_examples::Prod)
 B9_HANDLER(greet, b9_examples::Greet)
 B9_HANDLER(join, b9_examples::Join)
 B9_HANDLER(field_sum, b9_examples::FieldSum)
+B9_HANDLER(tokens, b9_examples::Tokens)
+B9_HANDLER(grid, b9_examples::Grid)
+B9_HANDLER(describe, b9_examples::Describe)
+B9_HANDLER(pick, b9_examples::Pick)

@@ -212,4 +212,99 @@ struct FieldSum {
     }
 };
 
+// ---- handlers that return lists and dicts -----------------------------------------------------------------------------
+// The words of the code points c[i, end) as strings of a list, split as str.split() does (WordCount::is_space)
+template <class Out> __device__ void put_words(const b9h::Chars& c, Out& out) {
+    b9h::Chars it = c;
+    bool in_word = false;
+    uint32_t cp;
+    out.list_begin();
+    while (it.next(cp)) {
+        const bool sp = WordCount::is_space(cp);
+        if (!sp && !in_word) out.str_begin();
+        if (sp && in_word) out.str_end();
+        if (!sp) out.cp(cp);
+        in_word = !sp;
+    }
+    if (in_word) out.str_end();
+    out.list_end();
+}
+
+// def tokens(s, /): return s.split()                     (a non-str has no .split: AttributeError)
+struct Tokens {
+    template <class Out> __device__ static int call(const b9h::Arg& s, Out& out) {
+        if (s.kind() != b9h::STR) return B9_EXC_ATTRIBUTE_ERROR;
+        put_words(s.chars(), out);
+        return 0;
+    }
+};
+
+// def grid(s, /): return [line.split() for line in s.split("\n")]
+// s.split("\n") splits on U+000A alone: one line more than the string has line feeds.
+struct Grid {
+    template <class Out> __device__ static int call(const b9h::Arg& s, Out& out) {
+        if (s.kind() != b9h::STR) return B9_EXC_ATTRIBUTE_ERROR;
+        b9h::Chars it = s.chars(), line = it;
+        uint32_t cp;
+        out.list_begin();
+        for (;;) {
+            const uint32_t at = it.i;
+            const bool more = it.next(cp);
+            if (more && cp != '\n') continue;
+            line.end = at;
+            put_words(line, out);
+            if (!more) break;
+            line.i = it.i;
+            line.end = it.end;
+        }
+        out.list_end();
+        return 0;
+    }
+};
+
+template <class Out> __device__ void put_key(const char* k, Out& out) { out.str_begin(); put_ascii(k, out); out.str_end(); }
+
+// def describe(x, /): return {"type": type(x).__name__, "value": x}
+struct Describe {
+    template <class Out> __device__ static int call(const b9h::Arg& x, Out& out) {
+        static const char* const names[] = {"str", "int", "float", "bool", "NoneType", "list", "dict"};
+        out.dict_begin();
+        put_key("type", out);
+        put_key(names[x.kind()], out);
+        put_key("value", out);
+        out.value(x);
+        out.dict_end();
+        return 0;
+    }
+};
+
+// def pick(d, /, *keys):
+//     if type(d) is not dict: raise TypeError
+//     return {k: d[k] for k in keys}
+// A list or dict key is unhashable (TypeError); any other key the dict lacks, a non-str one included, is KeyError. A
+// key given twice makes two equal keys in the built dict: the device declines it (UNSUPPORTED).
+struct Pick {
+    B9H_SIGNATURE(B9H_POS_ONLY("d"), B9H_VAR_POS("keys"));
+    template <class Out> __device__ static int call(const b9h::Call& c, Out& out) {
+        const b9h::Arg d = c[0];
+        if (d.kind() != b9h::DICT) return B9_EXC_TYPE_ERROR;
+        b9h::Items it = c.rest();
+        b9h::Arg k, v;
+        while (it.next(k)) {
+            const int kk = k.kind();
+            if (kk == b9h::LIST || kk == b9h::DICT) return B9_EXC_TYPE_ERROR;
+            if (!d.get(k, v)) return B9_EXC_KEY_ERROR;
+        }
+        out.dict_begin();
+        it = c.rest();
+        while (it.next(k)) {
+            d.get(k, v);
+            out.str_begin(); put_str(k, out); out.str_end();
+            out.value(v);
+        }
+        out.dict_end();
+        return 0;
+    }
+};
+
 }  // namespace b9_examples

@@ -51,5 +51,24 @@ def field_sum(rows, *, field):
     return total
 
 
+def tokens(s, /):
+    return s.split()
+
+
+def grid(s, /):
+    return [line.split() for line in s.split("\n")]
+
+
+def describe(x, /):
+    return {"type": type(x).__name__, "value": x}
+
+
+def pick(d, /, *keys):
+    if type(d) is not dict:
+        raise TypeError("pick picks from a dict")
+    return {k: d[k] for k in keys}
+
+
 TWINS = {"echo_str": echo_str, "crc32_str": crc32_str, "word_count": word_count, "prod": prod,
-         "greet": greet, "join": join, "field_sum": field_sum}
+         "greet": greet, "join": join, "field_sum": field_sum,
+         "tokens": tokens, "grid": grid, "describe": describe, "pick": pick}

@@ -41,17 +41,34 @@
 // positionals, a last "kwargs" object alone is the kwargs, else the body's other top-level keys are); a record's own.
 // Keywords match by decoded code points, the last of duplicate keys deciding. Arg::get reads a dict by key the same way.
 //
-// `call` runs twice for a string result: once with a counting sink (status, length, falsiness), then, once the warp has
-// reserved the record's bytes, with a writing sink. It must therefore be deterministic: a second pass that writes another
-// number of bytes than the first counted makes the record UNSUPPORTED, and the writing sink never writes past the
-// record's reservation. A number, bool or None result is written from the value the first pass stored.
+// The sink takes one value: none(), boolean(b), integer(i), real(d), a string (str_begin(), cp(c) per code point,
+// str_end()), an argument passed through (value(a): the bytes the built-in identity handler writes for it), or a
+// container. A list (list_begin() ... list_end()) holds any number of values; a dict (dict_begin() ... dict_end())
+// alternates a key, always a string, and its value:
+//
+//     out.dict_begin();                        // twin: return {"type": "str", "value": x}
+//     out.str_begin(); put("type"); out.str_end();  out.str_begin(); put("str"); out.str_end();
+//     out.str_begin(); put("value"); out.str_end(); out.value(x);
+//     out.dict_end();
+//
+// Containers nest at most 16 deep and a dict holds at most 64 members, with no two keys equal (Python would keep one).
+// Past those limits the record is UNSUPPORTED, as it is for a close that matches no open container, a non-string key,
+// a dict closed after its key, a container call inside an open string, a result left open, and a value(a) whose
+// argument identity declines (nesting past 16, more than 64 members, a number f64_parse cannot settle).
+//
+// `call` runs twice for a string, container or value() result: once with a counting sink (status, length, falsiness),
+// then, once the warp has reserved the record's bytes, with a writing sink. It must therefore be deterministic: a second
+// pass that writes another number of bytes than the first counted makes the record UNSUPPORTED, and the writing sink
+// never writes past the record's reservation. A number, bool or None result is written from the value the first pass
+// stored.
 //
 // The result is rendered as the runner would:
 //   b9_drain_launch            serialize_result(result) if result else None: json.dumps with its defaults (ensure_ascii,
-//                              NaN / Infinity written); a falsy result (None, False, 0, 0.0, -0.0, "") is COMPLETE
+//                              ", " and ": ", NaN / Infinity written, dict keys in the order written); a falsy result
+//                              (None, False, 0, 0.0, -0.0, "", [], {}, or a value() identity drops) is COMPLETE
 //                              without result bytes
 //   b9_endpoint_drain_launch   JSONResponse(result).body: compact, ensure_ascii=False, every result has a body; a
-//                              non-finite float is UNSUPPORTED (allow_nan=False raises)
+//                              non-finite float at any depth is UNSUPPORTED (allow_nan=False raises)
 // A string holding a surrogate or a code point above U+10FFFF is UNSUPPORTED in both.
 //
 // This header is plain C++ behind CUDA qualifiers up to the kernel, which only nvcc sees: a host test can compile a
@@ -98,6 +115,8 @@ struct Chars {
 
 class Arg;
 struct Items;
+template <int R> struct CountSink;
+template <int R> struct WriteSink;
 
 // A read-only view of one JSON value p[s, e) (validated) as the runner's json.loads made it. `unsure` is set when the
 // handler asked something the device cannot answer exactly (the int / float type of a number whose float64 f64_parse
@@ -144,8 +163,25 @@ public:
 
 private:
     friend class Call;
+    template <int> friend struct CountSink;
+    template <int> friend struct WriteSink;
     // number() without the range rule: *range = an int outside int64 (its kind is still INT)
     __device__ int num(long long* i, double* f, bool* range) const;
+    // the sinks' value(a): identity's bytes for the token in rendering R (o == nullptr: their count), -1 where
+    // py_value_json / ep_value_json decline
+    template <int R> __device__ int64_t json(uint8_t* o) const {
+        return R == ENDPOINT ? b9::ep_value_json(p_, s_, e_, o) : b9::py_value_json(p_, s_, e_, o);
+    }
+    // Python's truth value of the token: what the built-in identity handler drops as falsy
+    __device__ bool truthy() const {
+        switch (p_[s_]) {
+        case '"': return e_ - s_ > 2;
+        case 't': return true;
+        case 'n': case 'f': return false;
+        case '[': case '{': return !empty();
+        default: { unsigned long long b = 0; b9::f64_parse(p_, s_, e_, &b); return (b << 1) != 0; }
+        }
+    }
     const uint8_t* p_; uint32_t s_, e_; bool* unsure_;
 };
 
@@ -263,70 +299,13 @@ __device__ inline int Arg::num(long long* i, double* f, bool* range) const {
 }
 
 // ---- the sinks ------------------------------------------------------------------------------------------------------
-// What the first pass learns about the one value the handler writes
-enum ValueKind : uint8_t { VK_UNSET = 0, VK_NONE, VK_BOOL, VK_INT, VK_FLOAT, VK_STR, VK_BAD };
+// What the first pass learns about the one value the handler writes: VK_LIST / VK_DICT, a container it built;
+// VK_VALUE, an argument it passed through with value()
+enum ValueKind : uint8_t { VK_UNSET = 0, VK_NONE, VK_BOOL, VK_INT, VK_FLOAT, VK_STR, VK_BAD, VK_LIST, VK_DICT, VK_VALUE };
 
 template <int R> __device__ __forceinline__ uint32_t str_cp_len(uint32_t cp) { return R == ENDPOINT ? b9::ep_emit_len(cp) : b9::py_escaped_len(cp); }
 template <int R> __device__ __forceinline__ uint32_t str_cp_write(uint32_t cp, uint8_t* o) { return R == ENDPOINT ? b9::ep_emit(cp, o) : b9::py_emit(cp, o); }
 __device__ __forceinline__ bool cp_ok(uint32_t cp) { return cp <= 0x10FFFFu && (cp - 0xD800u) >= 0x800u; }
-
-// Pass 1: counts the string's bytes and keeps a number's value. vk = VK_BAD for anything the renderings cannot write:
-// a second value, a string left open, a surrogate or a code point past U+10FFFF.
-template <int R> struct CountSink {
-    uint8_t vk = VK_UNSET; bool open = false;
-    uint32_t n = 0, cps = 0;
-    long long v = 0;                 // VK_BOOL / VK_INT; VK_FLOAT: the double's bits
-    __device__ bool start(uint8_t k) { if (vk != VK_UNSET || open) { vk = VK_BAD; open = false; return false; } vk = k; return true; }
-    __device__ void none() { start(VK_NONE); }
-    __device__ void boolean(bool b) { if (start(VK_BOOL)) v = b ? 1 : 0; }
-    __device__ void integer(long long x) { if (start(VK_INT)) v = x; }
-    __device__ void real(double d) { if (start(VK_FLOAT)) v = (long long)b9::f64_to_bits(d); }
-    __device__ void str_begin() { if (start(VK_STR)) { open = true; n = 2; cps = 0; } }
-    __device__ void cp(uint32_t c) {
-        if (!open) { vk = VK_BAD; return; }
-        if (!cp_ok(c)) { vk = VK_BAD; open = false; return; }
-        n += str_cp_len<R>(c); ++cps;
-    }
-    __device__ void str_end() { if (!open) vk = VK_BAD; open = false; }
-};
-
-// Pass 2 of a string result: writes at most `cap` bytes at o
-template <int R> struct WriteSink {
-    uint8_t* o; uint32_t cap, n = 0; bool ok = true, open = false, done = false;
-    __device__ WriteSink(uint8_t* out, uint32_t c) : o(out), cap(c) {}
-    __device__ void bad() { ok = false; }
-    __device__ void none() { bad(); }
-    __device__ void boolean(bool) { bad(); }
-    __device__ void integer(long long) { bad(); }
-    __device__ void real(double) { bad(); }
-    __device__ void str_begin() { if (done || open || cap < 2) { bad(); return; } o[0] = '"'; n = 1; open = true; }
-    __device__ void cp(uint32_t c) {
-        if (!ok || !open || !cp_ok(c)) { bad(); return; }
-        if (n + str_cp_len<R>(c) + 1 > cap) { bad(); return; }       // (+1: the closing quote)
-        n += str_cp_write<R>(c, o + n);
-    }
-    __device__ void str_end() { if (!ok || !open) { bad(); return; } o[n++] = '"'; open = false; done = true; }
-};
-
-// ---- phase A and B around a handler ---------------------------------------------------------------------------------
-struct UserRec {
-    uint32_t src_off, src_len;   // args[0]'s token: pass 2 of a string result calls the handler on it again
-    uint32_t out_len;
-    uint8_t status, has, vk;
-    long long value;             // ERROR: the exception class (one B9_EXC_* bit); else the number pass 1 stored
-};
-
-// The tasks a rendering answers, parsed: task-queue: an SDK payload (flags 0), an HTTP body (B9_TF_HTTP_BODY) or a
-// TaskMessage record of the slot's id (B9_TF_TASK_MSG); endpoint: exactly B9_TF_HTTP_BODY (endpoint_accepts). Anything
-// else (B9_TF_PICKLE, combinations) is UNSUPPORTED. `id`: the slot's 16 raw id bytes (read only for a record).
-template <int R> __device__ inline b9::Parsed user_parse(const uint8_t* p, uint32_t n, uint32_t flags, const uint8_t* id) {
-    b9::Parsed pr;
-    if (R == ENDPOINT ? b9::endpoint_accepts(flags) : (flags == 0 || flags == B9_TF_HTTP_BODY)) return b9::parse_payload(p, n, flags != 0);
-    if (R == TASK_QUEUE && flags == B9_TF_TASK_MSG) return b9::parse_task_msg(p, n, id);
-    pr.status = b9::ST_UNSUPPORTED; pr.nargs = 0; pr.a0_off = pr.a0_len = 0;
-    return pr;
-}
-
 // record length of a number / bool / None result (o == nullptr), or its bytes
 template <int R> __device__ inline uint32_t scalar_write(uint8_t vk, long long v, uint8_t* o) {
     switch (vk) {
@@ -344,6 +323,236 @@ template <int R> __device__ inline uint32_t scalar_write(uint8_t vk, long long v
     }
 }
 
+__device__ __forceinline__ bool nonfinite(long long bits) { return (((unsigned long long)bits >> 52) & 0x7FFull) == 0x7FFull; }
+// the separators of a rendering: json.dumps's ", " and ": ", JSONResponse's "," and ":"
+template <int R> __host__ __device__ constexpr uint32_t sep_len() { return R == ENDPOINT ? 1u : 2u; }
+
+// Containers (list_begin ... list_end, dict_begin ... dict_end) nest at most PY_VALUE_MAX_DEPTH deep. Both sinks keep
+// one bit per open container, bit d for depth d: `dict` (a dict, else a list), `started` (an item or member written:
+// the next one needs a separator) and `keyed` (a dict whose key is written and whose value is due). A dict's members
+// alternate a str key (str_begin / cp / str_end) and a value; key_open: the open string is a key.
+
+// Pass 1: counts the result's bytes and keeps a number's value. vk = VK_BAD for anything the renderings cannot write:
+// a second value, a string or container left open, a surrogate or a code point past U+10FFFF, a close that matches no
+// open container, a key that is not a string, a dict closed after a key, a 17th open container, a value() its
+// rendering declines, a non-finite float inside a container of the endpoint rendering.
+template <int R> struct CountSink {
+    uint8_t vk = VK_UNSET; bool open = false;
+    uint32_t n = 0, cps = 0;
+    long long v = 0;                 // VK_BOOL / VK_INT; VK_FLOAT: the double's bits
+    int depth = 0; uint32_t dict = 0, started = 0, keyed = 0; bool key_open = false;
+    bool truthy = false;             // VK_LIST / VK_DICT / VK_VALUE: the result is not empty (falsy)
+    __device__ bool start(uint8_t k) { if (vk != VK_UNSET || open) { vk = VK_BAD; open = false; return false; } vk = k; return true; }
+    // a value or key begins inside the innermost container; false when that breaks a rule (vk is then VK_BAD)
+    __device__ bool item(bool str) {
+        if (vk == VK_BAD) return false;
+        const uint32_t bit = 1u << (depth - 1);
+        if (open || ((dict & bit) && !(keyed & bit) && !str)) { vk = VK_BAD; open = false; return false; }
+        if (keyed & bit) { keyed &= ~bit; n += sep_len<R>(); return true; }
+        if (started & bit) n += sep_len<R>();
+        started |= bit;
+        key_open = (dict & bit) != 0;
+        return true;
+    }
+    __device__ void scalar(uint8_t k, long long x) {
+        if (!item(false)) return;
+        if (R == ENDPOINT && k == VK_FLOAT && nonfinite(x)) { vk = VK_BAD; return; }      // allow_nan=False
+        n += scalar_write<R>(k, x, nullptr);
+    }
+    __device__ void none() { if (depth) scalar(VK_NONE, 0); else start(VK_NONE); }
+    __device__ void boolean(bool b) { if (depth) scalar(VK_BOOL, b ? 1 : 0); else if (start(VK_BOOL)) v = b ? 1 : 0; }
+    __device__ void integer(long long x) { if (depth) scalar(VK_INT, x); else if (start(VK_INT)) v = x; }
+    __device__ void real(double d) {
+        if (depth) scalar(VK_FLOAT, (long long)b9::f64_to_bits(d));
+        else if (start(VK_FLOAT)) v = (long long)b9::f64_to_bits(d);
+    }
+    __device__ void str_begin() {
+        if (depth) { if (item(true)) { open = true; n += 2; } return; }
+        if (start(VK_STR)) { open = true; n = 2; cps = 0; }
+    }
+    __device__ void cp(uint32_t c) {
+        if (!open) { vk = VK_BAD; return; }
+        if (!cp_ok(c)) { vk = VK_BAD; open = false; return; }
+        n += str_cp_len<R>(c); ++cps;
+    }
+    __device__ void str_end() {
+        if (!open) vk = VK_BAD;
+        else if (key_open) { keyed |= 1u << (depth - 1); key_open = false; }
+        open = false;
+    }
+    __device__ void begin(uint8_t k) {
+        if (depth) { if (!item(false)) return; }
+        else if (!start(k)) return;
+        if (depth == b9::PY_VALUE_MAX_DEPTH) { vk = VK_BAD; return; }
+        const uint32_t bit = 1u << depth;
+        dict = k == VK_DICT ? dict | bit : dict & ~bit; started &= ~bit; keyed &= ~bit;
+        ++depth; ++n;
+    }
+    __device__ void end(uint8_t k) {
+        if (vk == VK_BAD) return;
+        const uint32_t bit = depth ? 1u << (depth - 1) : 0u;
+        if (open || !depth || ((dict & bit) != 0) != (k == VK_DICT) || (keyed & bit)) { vk = VK_BAD; open = false; return; }
+        --depth; ++n;
+        if (!depth) truthy = (started & 1u) != 0;
+    }
+    __device__ void list_begin() { begin(VK_LIST); }
+    __device__ void list_end() { end(VK_LIST); }
+    __device__ void dict_begin() { begin(VK_DICT); }
+    __device__ void dict_end() { end(VK_DICT); }
+    __device__ void value(const Arg& a) {
+        if (depth) { if (!item(false)) return; }
+        else if (!start(VK_VALUE)) return;
+        const int64_t l = a.json<R>(nullptr);
+        if (l < 0) { vk = VK_BAD; return; }
+        n += (uint32_t)l;
+        if (!depth) truthy = a.truthy();
+    }
+};
+
+// Pass 2 of a string, container or value() result: writes at most `cap` bytes at o. A number, bool or None is written
+// only inside a container (at the top level, from the value pass 1 stored). dict_end checks the member keys it has
+// just written: more than PY_VALUE_MAX_MEMBERS, or two equal ones (the writers are canonical: equal bytes are equal
+// code points), fail the pass.
+template <int R> struct WriteSink {
+    uint8_t* o; uint32_t cap, n = 0; bool ok = true, open = false, done = false;
+    int depth = 0; uint32_t dict = 0, started = 0, keyed = 0; bool key_open = false;
+    uint32_t at[b9::PY_VALUE_MAX_DEPTH];     // where each open container's bracket is
+    __device__ WriteSink(uint8_t* out, uint32_t c) : o(out), cap(c) {}
+    __device__ void bad() { ok = false; }
+    __device__ bool room(uint32_t l) { if (n + l > cap) { bad(); return false; } return true; }
+    __device__ bool item(bool str) {
+        const uint32_t bit = 1u << (depth - 1);
+        if (!ok || open || ((dict & bit) && !(keyed & bit) && !str)) { bad(); return false; }
+        if ((keyed & bit) || (started & bit)) {
+            if (!room(sep_len<R>())) return false;
+            o[n] = (keyed & bit) ? ':' : ',';
+            if (R == TASK_QUEUE) o[n + 1] = ' ';
+            n += sep_len<R>();
+            if (keyed & bit) { keyed &= ~bit; return true; }
+        }
+        started |= bit;
+        key_open = (dict & bit) != 0;
+        return true;
+    }
+    __device__ void scalar(uint8_t k, long long x) {
+        if (!depth) { bad(); return; }
+        if (!item(false)) return;
+        if (R == ENDPOINT && k == VK_FLOAT && nonfinite(x)) { bad(); return; }
+        if (room(scalar_write<R>(k, x, nullptr))) n += scalar_write<R>(k, x, o + n);
+    }
+    __device__ void none() { scalar(VK_NONE, 0); }
+    __device__ void boolean(bool b) { scalar(VK_BOOL, b ? 1 : 0); }
+    __device__ void integer(long long x) { scalar(VK_INT, x); }
+    __device__ void real(double d) { scalar(VK_FLOAT, (long long)b9::f64_to_bits(d)); }
+    __device__ void str_begin() {
+        if (depth) { if (item(true) && room(2)) { o[n++] = '"'; open = true; } return; }     // (2: the closing quote)
+        if (done || open || cap < 2) { bad(); return; } o[0] = '"'; n = 1; open = true;
+    }
+    __device__ void cp(uint32_t c) {
+        if (!ok || !open || !cp_ok(c)) { bad(); return; }
+        if (n + str_cp_len<R>(c) + 1 > cap) { bad(); return; }       // (+1: the closing quote)
+        n += str_cp_write<R>(c, o + n);
+    }
+    __device__ void str_end() {
+        if (!ok || !open) { bad(); return; }
+        o[n++] = '"'; open = false;
+        if (!depth) done = true;
+        else if (key_open) { keyed |= 1u << (depth - 1); key_open = false; }
+    }
+    __device__ void begin(bool is_dict) {
+        if (depth) { if (!item(false)) return; }
+        else if (done || open) { bad(); return; }
+        if (depth == b9::PY_VALUE_MAX_DEPTH || !room(1)) { bad(); return; }
+        const uint32_t bit = 1u << depth;
+        dict = is_dict ? dict | bit : dict & ~bit; started &= ~bit; keyed &= ~bit;
+        at[depth++] = n;
+        o[n++] = is_dict ? '{' : '[';
+    }
+    __device__ void end(bool is_dict) {
+        const uint32_t bit = depth ? 1u << (depth - 1) : 0u;
+        if (!ok || open || !depth || ((dict & bit) != 0) != is_dict || (keyed & bit)) { bad(); return; }
+        if (is_dict && !keys_ok(at[depth - 1] + 1)) { bad(); return; }
+        if (!room(1)) return;
+        o[n++] = is_dict ? '}' : ']';
+        if (!--depth) done = true;
+    }
+    __device__ void list_begin() { begin(false); }
+    __device__ void list_end() { end(false); }
+    __device__ void dict_begin() { begin(true); }
+    __device__ void dict_end() { end(true); }
+    __device__ void value(const Arg& a) {
+        if (depth) { if (!item(false)) return; }
+        else if (done || open) { bad(); return; }
+        const int64_t l = a.json<R>(nullptr);
+        if (l < 0 || !room((uint32_t)l)) { bad(); return; }
+        n += (uint32_t)a.json<R>(o + n);
+        if (!depth) done = true;
+    }
+
+    // the bytes this sink wrote: one string o[i] == '"' ... (past its closing quote), one value (to the ',' or the end e
+    // that follows it), the next member key of a dict body (i: its start or the end of a value; [ks, ke): between the
+    // quotes; false at e)
+    __device__ uint32_t skip_str(uint32_t i, uint32_t e) const {
+        for (++i; i < e && o[i] != '"'; ++i) if (o[i] == '\\') ++i;
+        return i + 1;
+    }
+    __device__ uint32_t skip_value(uint32_t i, uint32_t e) const {
+        int d = 0;
+        while (i < e) {
+            const uint8_t c = o[i];
+            if (c == '"') { i = skip_str(i, e); continue; }
+            if (c == '[' || c == '{') ++d;
+            else if (c == ']' || c == '}') --d;
+            else if (c == ',' && d == 0) return i;
+            ++i;
+        }
+        return i;
+    }
+    __device__ bool next_key(uint32_t& i, uint32_t e, uint32_t& ks, uint32_t& ke) const {
+        while (i < e && (o[i] == ',' || o[i] == ' ')) ++i;
+        if (i >= e) return false;
+        ks = i + 1;
+        i = skip_str(i, e);
+        ke = i - 1;
+        i = skip_value(i + sep_len<R>(), e);
+        return true;
+    }
+    // the members of the dict body o[s, n): at most PY_VALUE_MAX_MEMBERS, no two keys equal
+    __device__ bool keys_ok(uint32_t s) const {
+        uint32_t i = s, ks, ke, members = 0;
+        while (next_key(i, n, ks, ke)) {
+            if (++members > b9::PY_VALUE_MAX_MEMBERS) return false;
+            uint32_t j = s, js, je;
+            while (next_key(j, ks - 1, js, je)) {
+                if (je - js != ke - ks) continue;
+                uint32_t k = 0;
+                while (k < ke - ks && o[js + k] == o[ks + k]) ++k;
+                if (k == ke - ks) return false;
+            }
+        }
+        return true;
+    }
+};
+
+// ---- phase A and B around a handler ---------------------------------------------------------------------------------
+struct UserRec {
+    uint32_t src_off, src_len;   // args[0]'s token: pass 2 of a string or container result calls the handler on it again
+    uint32_t out_len;
+    uint8_t status, has, vk;
+    long long value;             // ERROR: the exception class (one B9_EXC_* bit); else the number pass 1 stored
+};
+
+// The tasks a rendering answers, parsed: task-queue: an SDK payload (flags 0), an HTTP body (B9_TF_HTTP_BODY) or a
+// TaskMessage record of the slot's id (B9_TF_TASK_MSG); endpoint: exactly B9_TF_HTTP_BODY (endpoint_accepts). Anything
+// else (B9_TF_PICKLE, combinations) is UNSUPPORTED. `id`: the slot's 16 raw id bytes (read only for a record).
+template <int R> __device__ inline b9::Parsed user_parse(const uint8_t* p, uint32_t n, uint32_t flags, const uint8_t* id) {
+    b9::Parsed pr;
+    if (R == ENDPOINT ? b9::endpoint_accepts(flags) : (flags == 0 || flags == B9_TF_HTTP_BODY)) return b9::parse_payload(p, n, flags != 0);
+    if (R == TASK_QUEUE && flags == B9_TF_TASK_MSG) return b9::parse_task_msg(p, n, id);
+    pr.status = b9::ST_UNSUPPORTED; pr.nargs = 0; pr.a0_off = pr.a0_len = 0;
+    return pr;
+}
+
 // What `call` returned (ret), whether it asked something the device cannot answer (unsure) and what it wrote (out) as
 // the record's status, has and length: the rules of user_phase_a below, for a handler with a signature (user_phase_a
 // keeps its own copy so that the one-Arg entries compile to the same code as before signatures existed).
@@ -354,17 +563,18 @@ template <int R> __device__ inline bool phase_a_settle(int ret, bool unsure, con
         if (ret > 0 && ret <= (int)B9_EXC_ALL && !(ret & (ret - 1))) { rec.status = b9::ST_ERROR; rec.value = ret; }
         return false;
     }
-    if (out.vk == VK_UNSET || out.vk == VK_BAD || out.open) return false;
+    if (out.vk == VK_UNSET || out.vk == VK_BAD || out.open || out.depth) return false;
     if (out.vk == VK_FLOAT && R == ENDPOINT && (((unsigned long long)out.v >> 52) & 0x7FFull) == 0x7FFull) return false;   // allow_nan=False
     rec.status = b9::ST_OK;
     rec.vk = out.vk; rec.value = out.v;
     if (R == TASK_QUEUE) {                                        // `serialize_result(result) if result else None`
         const bool falsy = out.vk == VK_NONE || ((out.vk == VK_BOOL || out.vk == VK_INT) && out.v == 0) ||
-                           (out.vk == VK_FLOAT && ((unsigned long long)out.v << 1) == 0) || (out.vk == VK_STR && out.cps == 0);
+                           (out.vk == VK_FLOAT && ((unsigned long long)out.v << 1) == 0) || (out.vk == VK_STR && out.cps == 0) ||
+                           (out.vk >= VK_LIST && !out.truthy);
         if (falsy) return false;
     }
     rec.has = 1;
-    rec.out_len = out.vk == VK_STR ? out.n : scalar_write<R>(out.vk, out.v, nullptr);
+    rec.out_len = out.vk >= VK_STR ? out.n : scalar_write<R>(out.vk, out.v, nullptr);
     return true;
 }
 
@@ -383,24 +593,25 @@ template <class H, int R> __device__ inline void user_phase_a(const uint8_t* p, 
         if (ret > 0 && ret <= (int)B9_EXC_ALL && !(ret & (ret - 1))) { rec.status = b9::ST_ERROR; rec.value = ret; }
         return;
     }
-    if (out.vk == VK_UNSET || out.vk == VK_BAD || out.open) return;
+    if (out.vk == VK_UNSET || out.vk == VK_BAD || out.open || out.depth) return;
     if (out.vk == VK_FLOAT && R == ENDPOINT && (((unsigned long long)out.v >> 52) & 0x7FFull) == 0x7FFull) return;   // allow_nan=False
     rec.status = b9::ST_OK;
     rec.vk = out.vk; rec.value = out.v;
     if (R == TASK_QUEUE) {                                        // `serialize_result(result) if result else None`
         const bool falsy = out.vk == VK_NONE || ((out.vk == VK_BOOL || out.vk == VK_INT) && out.v == 0) ||
-                           (out.vk == VK_FLOAT && ((unsigned long long)out.v << 1) == 0) || (out.vk == VK_STR && out.cps == 0);
+                           (out.vk == VK_FLOAT && ((unsigned long long)out.v << 1) == 0) || (out.vk == VK_STR && out.cps == 0) ||
+                           (out.vk >= VK_LIST && !out.truthy);
         if (falsy) return;
     }
     rec.has = 1;
     rec.src_off = pr.a0_off; rec.src_len = pr.a0_len;
-    rec.out_len = out.vk == VK_STR ? out.n : scalar_write<R>(out.vk, out.v, nullptr);
+    rec.out_len = out.vk >= VK_STR ? out.n : scalar_write<R>(out.vk, out.v, nullptr);
 }
 
 // Phase B: writes the record's rec.out_len bytes at o. false: the handler's second pass did not write what its first
 // counted (the bytes at o are then not a record, and the caller makes it UNSUPPORTED).
 template <class H, int R> __device__ inline bool user_phase_b(const uint8_t* p, const UserRec& rec, uint8_t* o) {
-    if (rec.vk != VK_STR) { scalar_write<R>(rec.vk, rec.value, o); return true; }
+    if (rec.vk < VK_STR) { scalar_write<R>(rec.vk, rec.value, o); return true; }
     bool unsure = false;
     const Arg arg(p, rec.src_off, rec.src_off + rec.src_len, &unsure);
     WriteSink<R> out(o, rec.out_len);
@@ -574,7 +785,7 @@ __device__ inline CallSrc call_src(const uint8_t* p, uint32_t n, uint32_t flags,
 }
 
 struct CallRec : UserRec {
-    CallSrc src;                 // pass 2 of a string result binds the call again from here
+    CallSrc src;                 // pass 2 of a string or container result binds the call again from here
 };
 
 // Phase A of a handler with a signature. A task-queue SDK payload whose "kwargs" came more than once as objects (Go
@@ -594,7 +805,7 @@ template <class H, int R> __device__ inline void call_phase_a(const uint8_t* p, 
 }
 
 template <class H, int R> __device__ inline bool call_phase_b(const uint8_t* p, const CallRec& rec, uint8_t* o) {
-    if (rec.vk != VK_STR) { scalar_write<R>(rec.vk, rec.value, o); return true; }
+    if (rec.vk < VK_STR) { scalar_write<R>(rec.vk, rec.value, o); return true; }
     bool unsure = false;
     Call c;
     if (!c.bind<H>(p, rec.src, &unsure)) return false;
